@@ -3,7 +3,8 @@ oracle/_ref by build(), which is only possible where the reference source tree i
 tests/test_ref_pinning.py, which compares the oracle and the Python mirror against them, and the results of the
 reference's own runner file (src/limap/runners/line_triangulation.py) on the scene of tests/test_runner_dropin.py.
 
-Run from the repository root:  python tests/golden/make_ref_golden.py"""
+Run from the repository root:  python tests/golden/make_ref_golden.py [name ...]
+(no names: every file; names: only tests/golden/ref/<name>.npz)"""
 import os
 import sys
 
@@ -24,7 +25,12 @@ def main():
     os.makedirs(t.GOLD, exist_ok=True)
     runner = os.path.join(ref.REFERENCE_SRC, "limap", "runners", "line_triangulation.py")
     outputs = dict(t.REFERENCE_OUTPUTS, runner_line_triangulation=lambda: rd.reference_runner_outputs(runner))
-    for name, make in outputs.items():
+    names = sys.argv[1:] or list(outputs)
+    unknown = sorted(set(names) - set(outputs))
+    if unknown:
+        raise SystemExit(f"unknown golden files: {unknown}")
+    for name in names:
+        make = outputs[name]
         path = os.path.join(t.GOLD, name + ".npz")
         np.savez_compressed(path, **make())
         print(f"{path}: {os.path.getsize(path)} bytes")

@@ -7,10 +7,26 @@ ENDPOINT_TOL = 1e-4   # BASELINE.json north_star: "within 1e-4 absolute on 3D li
 SCORE_TOL = 1e-6
 
 
-def run_both(scene, cfg, exhaustive=False, use_ranges=True, vpresults=None):
+def fake_vpresults(sc, seed):
+    """Random but well-formed VPResults: ~60% of the lines of every image carry one of 3 VPs."""
+    from limap_b200.vplib import VPResult
+    rng = np.random.default_rng(seed)
+    out = {}
+    for v, i in enumerate(sc.img_ids):
+        L = int(sc.line_off[v + 1] - sc.line_off[v])
+        vps = rng.normal(size=(3, 3))
+        vps[:, :2] *= 1000.0
+        vps /= np.linalg.norm(vps, axis=1, keepdims=True)
+        labels = rng.integers(0, 3, L)
+        labels[rng.random(L) < 0.4] = -1
+        out[int(i)] = VPResult(labels, vps)
+    return out
+
+
+def run_both(scene, cfg, exhaustive=False, use_ranges=True, vpresults=None, node_parallel=False):
     from limap_b200.engine import TriEngine
     from oracle.oracle import OracleTri
-    eng, orc = TriEngine(cfg), OracleTri(cfg)
+    eng, orc = TriEngine(cfg), OracleTri(cfg, node_parallel=node_parallel)
     for t in (eng, orc):
         t.upload(scene)
         if use_ranges:

@@ -6,8 +6,12 @@ is available), so the pinning runs anywhere. Where an input set is large, the re
 sample of it (every k-th item) and the oracle still runs on the whole set.
 
   * whole pipeline: limap::triangulation::GlobalLineTriangulator (Init -> TriangulateImage -> ComputeLineTracks) against
-    OracleTri on seeded scenes and every configuration family the GPU tests use -- candidate lists, scores, valid
-    connections, best candidates, graph-ordered track membership bit-exact, coordinates to 1e-9;
+    OracleTri on seeded scenes and the configuration families the GPU tests use (the GPU configuration matrix also moves
+    single thresholds -- score_th, min_length_2d, the phase-A angle and sensitivity cut-offs -- around the families
+    pinned here) -- candidate lists, scores, valid connections, best candidates, graph-ordered track membership
+    bit-exact, coordinates to 1e-9;
+  * decision boundaries (tests/boundary_scenes.py): 2D lengths equal to min_length_2d, 3D angles and scale-invariant
+    distances planted at threshold * (1 -+ delta) for delta 1e-6, 1e-9, 1e-11;
   * function level on 2e4..1e5 random inputs each: compute_epipolar_IoU, triangulate_line (plane pair and endpoints),
     triangulate_line_with_direction, LineLinker2d/3d::compute_score, Line3d::sensitivity / computeUncertainty,
     CameraView::projection / ray_direction, Aggregator::aggregate_line3d_list, MinimalInfiniteLine3d,
@@ -83,6 +87,20 @@ CASES = {
     "exhaustive": (dict(V=5, L=40, N=3, K=2, seed=207), {}, dict(exhaustive=True)),
     "vp_proposals": (dict(V=6, L=60, N=4, K=3, seed=208), dict(use_vp=True), dict(vp=9)),
     "innerseg_2d_linker": (dict(V=6, L=80, N=4, K=4, seed=209), dict(linker2d_config=dict(use_innerseg=True, th_innerseg=3.0)), {}),
+    # sub-tests of both linkers switched off or moved: no perpendicular / smart-angle test, 2D and 3D angles above the
+    # 14.4775 deg switch of the asin^2 series, other score thresholds and scale invariance
+    "linker_flag_variants": (dict(V=7, L=80, N=4, K=4, seed=210), dict(
+        linker2d_config=dict(DEFAULT_YAML_TRIANGULATION["linker2d_config"], use_perp=False, use_smartangle=False,
+                             th_angle=20.0, score_th=0.3),
+        linker3d_config=dict(DEFAULT_YAML_TRIANGULATION["linker3d_config"], th_angle=20.0, th_scaleinv=0.05,
+                             score_th=0.8)), {}),
+    "linker_no_overlap_no_angle": (dict(V=7, L=80, N=4, K=4, seed=211), dict(
+        linker2d_config=dict(DEFAULT_YAML_TRIANGULATION["linker2d_config"], use_overlap=False, use_angle=False),
+        linker3d_config=dict(DEFAULT_YAML_TRIANGULATION["linker3d_config"], th_angle=90.0, th_scaleinv=0.002)), {}),
+    # the gates of phase A at their off values, and the rank of every candidate deciding the valid connections
+    "phase_a_gates_off": (dict(V=7, L=80, N=4, K=4, seed=212), dict(
+        line_tri_angle_threshold=0.0, sensitivity_threshold=90.0, IoU_threshold=0.0, min_length_2d=-1.0), {}),
+    "rank_all_valid": (dict(V=6, L=60, N=5, K=6, seed=213), dict(fullscore_th=0.0, max_valid_conns=2), {}),
 }
 
 
@@ -99,8 +117,9 @@ def _pipeline_case(name):
 CAND_LINES_EVERY = 2  # candidate ids are stored for every node, candidate coordinates for every 2nd node
 
 
-def _record_tri(t, sc):
-    """Everything compare_nodes / compare_tracks read from a triangulator, as flat arrays."""
+def _record_tri(t, sc, every=CAND_LINES_EVERY):
+    """Everything compare_nodes / compare_tracks read from a triangulator, as flat arrays (candidate coordinates of
+    every `every`-th node)."""
     best, ng, nc, ecnt, edges, ccnt, cline, cng = [], [], [], [], [], [], [], []
     for i in sc.img_ids:
         l, g, c = t.get_best(int(i))
@@ -110,7 +129,7 @@ def _record_tri(t, sc):
         for k in range(len(c)):
             cl, cg = t.get_cands_node(int(i), k)
             ccnt.append(len(cl)); cng.append(cg.reshape(-1, 2))
-            if (len(ccnt) - 1) % CAND_LINES_EVERY == 0:
+            if (len(ccnt) - 1) % every == 0:
                 cline.append(cl.reshape(-1, 10))
     out = dict(best_line=np.concatenate(best), best_ng=np.concatenate(ng), best_nc=np.concatenate(nc),
                edge_cnt=np.concatenate(ecnt), edges=np.concatenate(edges).astype(np.int32),
@@ -122,14 +141,14 @@ def _record_tri(t, sc):
 class _StoredTri:
     """The reference triangulator's answers, replayed from _record_tri's arrays."""
 
-    def __init__(self, z, sc):
-        self.z = z
+    def __init__(self, z, sc, every=CAND_LINES_EVERY):
+        self.z, self.every = z, every
         n = np.diff(sc.line_off)
         self.first = {int(i): int(o) for i, o in zip(sc.img_ids, np.concatenate([[0], np.cumsum(n)]))}
         self.n = {int(i): int(k) for i, k in zip(sc.img_ids, n)}
         self.eoff = np.concatenate([[0], np.cumsum(z["edge_cnt"])]).astype(np.int64)
         self.coff = np.concatenate([[0], np.cumsum(z["cand_cnt"])]).astype(np.int64)
-        self.loff = np.concatenate([[0], np.cumsum(z["cand_cnt"][::CAND_LINES_EVERY])]).astype(np.int64)
+        self.loff = np.concatenate([[0], np.cumsum(z["cand_cnt"][::every])]).astype(np.int64)
 
     def get_best(self, i):
         a, b = self.first[i], self.first[i] + self.n[i]
@@ -145,8 +164,8 @@ class _StoredTri:
         n = self.first[i] + l
         a, b = self.coff[n], self.coff[n + 1]
         lines = None
-        if n % CAND_LINES_EVERY == 0:
-            k = n // CAND_LINES_EVERY
+        if n % self.every == 0:
+            k = n // self.every
             lines = self.z["cand_line"][self.loff[k]:self.loff[k + 1]]
         return lines, self.z["cand_ng"][a:b]
 
@@ -159,29 +178,73 @@ def _ref_pipeline(name):
     return _record_tri(_feed(ref.RefTri(cfg, threads=1), sc, **run), sc)
 
 
-@pytest.mark.parametrize("name", sorted(CASES))
-def test_whole_pipeline_oracle_equals_compiled_reference(name, capfd):
-    sc, cfg, run = _pipeline_case(name)
-    o = _feed(orc.OracleTri(cfg, threads=1), sc, **run)
-    r = _StoredTri(_gold("pipeline_" + name), sc)
+def compare_stored(sc, r, o, endpoint_tol, score_tol=1e-9):
+    """The stored reference `r` against a triangulator `o`: candidate lists in reference order, valid connections, best
+    candidates and graph-ordered tracks bit-exact; coordinates within endpoint_tol, scores within score_tol."""
     import parity_utils
     old = parity_utils.ENDPOINT_TOL, parity_utils.SCORE_TOL
-    parity_utils.ENDPOINT_TOL, parity_utils.SCORE_TOL = 1e-7 * (100.0 if CASES[name][0].get("scale") else 1.0), 1e-9
+    parity_utils.ENDPOINT_TOL, parity_utils.SCORE_TOL = endpoint_tol, score_tol
     try:
         st = compare_nodes(sc, r, o)  # scores, valid connections, best candidates
-        assert st["candidates"] > 200 and st["valid_edges"] > 20
         for i in sc.img_ids:  # candidate lists in reference order
             for l in range(r.n[int(i)]):
                 cl, cng = r.get_cands_node(int(i), l)
                 ol, ong = o.get_cands_node(int(i), l)
                 assert np.array_equal(cng, ong), f"candidate list differs at node ({i},{l})"
                 if cl is not None and len(ol):
-                    assert np.abs(cl[:, :9] - ol[:, :9]).max() <= parity_utils.ENDPOINT_TOL
-                    assert np.abs(cl[:, 9] - ol[:, 9]).max() <= parity_utils.SCORE_TOL
+                    assert np.abs(cl[:, :9] - ol[:, :9]).max() <= endpoint_tol
+                    assert np.abs(cl[:, 9] - ol[:, 9]).max() <= score_tol
         tr = compare_tracks(r, o)
-        assert tr["tracks"] > 5 and tr["exact_order"]
+        assert tr["exact_order"]
     finally:
         parity_utils.ENDPOINT_TOL, parity_utils.SCORE_TOL = old
+    return dict(st, tracks=tr["tracks"])
+
+
+@pytest.mark.parametrize("name", sorted(CASES))
+def test_whole_pipeline_oracle_equals_compiled_reference(name, capfd):
+    sc, cfg, run = _pipeline_case(name)
+    o = _feed(orc.OracleTri(cfg, threads=1), sc, **run)
+    r = _StoredTri(_gold("pipeline_" + name), sc)
+    st = compare_stored(sc, r, o, 1e-7 * (100.0 if CASES[name][0].get("scale") else 1.0))
+    assert st["candidates"] > 200 and st["valid_edges"] > 20 and st["tracks"] > 5
+
+
+def _ref_boundary_min_length():
+    from boundary_scenes import min_length_cfg, min_length_scene
+    sc, _ = min_length_scene()
+    return _record_tri(_feed(ref.RefTri(min_length_cfg(), threads=1), sc), sc, every=1)
+
+
+def _ref_boundary_3d(name):
+    from boundary_scenes import boundary_3d_cfg, boundary_3d_scene
+    sc, _ = boundary_3d_scene(name)
+    return _record_tri(_feed(ref.RefTri(boundary_3d_cfg(name), threads=1), sc), sc, every=1)
+
+
+@pytest.mark.parametrize("name", ["angle_10", "angle_14.4775", "angle_20", "scaleinv"])
+def test_boundary_3d_oracle_equals_compiled_reference(name):
+    """3D angle and scale-invariant endpoint distance planted at threshold * (1 -+ delta), delta 1e-6 / 1e-9 / 1e-11,
+    at depths ~1 and ~1e3 and at asset-unit coordinates (tests/boundary_scenes.py): the reference's compiled code scores
+    the +delta pairs 0 and the -delta pairs >= score_th, and the oracle reproduces it."""
+    from boundary_scenes import boundary_3d_cfg, check_planted, checked_boundary_3d_scene
+    sc, planted = checked_boundary_3d_scene(name)
+    o = _feed(orc.OracleTri(boundary_3d_cfg(name), threads=1), sc)
+    r = _StoredTri(_gold("boundary_3d_" + name), sc, every=1)
+    check_planted(r, sc, planted)
+    compare_stored(sc, r, o, 1e-7)
+
+
+def test_boundary_min_length_oracle_equals_compiled_reference():
+    """2D segments of length exactly min_length_2d, as source lines and as matched lines: rejected by `<=`."""
+    from boundary_scenes import min_length_cfg, min_length_scene
+    sc, planted = min_length_scene()
+    o = _feed(orc.OracleTri(min_length_cfg(), threads=1), sc)
+    r = _StoredTri(_gold("boundary_min_length"), sc, every=1)
+    st = compare_stored(sc, r, o, 1e-7)
+    assert st["candidates"] > 1000
+    nc = np.concatenate([r.get_best(int(i))[2] for i in sc.img_ids])
+    assert (nc[planted] == 0).all()
 
 
 # ---- function level --------------------------------------------------------------------------------------------
@@ -977,6 +1040,9 @@ def test_camera_set_max_image_dim_rounding():
 
 # golden file name -> the reference's outputs on this module's inputs (tests/golden/make_ref_golden.py)
 REFERENCE_OUTPUTS = {**{"pipeline_" + name: (lambda name=name: _ref_pipeline(name)) for name in CASES},
+                     "boundary_min_length": _ref_boundary_min_length,
+                     **{"boundary_3d_" + name: (lambda name=name: _ref_boundary_3d(name))
+                        for name in ("angle_10", "angle_14.4775", "angle_20", "scaleinv")},
                      "two_view": _ref_two_view, "camera": _ref_camera, "linker": _ref_linker, "aggregate": _ref_aggregate,
                      "residuals": _ref_residuals, "filters": _ref_filters, "sfm": _ref_sfm, "vp": _ref_vp,
                      "linetrack": _ref_linetrack, "value_types": _ref_value_types, "track_filters": _ref_track_filters,

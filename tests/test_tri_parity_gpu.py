@@ -5,7 +5,7 @@ import pytest
 from limap_b200.config import DEFAULT_YAML_TRIANGULATION
 from limap_b200.synth import make_scene
 
-from parity_utils import compare_nodes, compare_tracks, run_both
+from parity_utils import compare_nodes, compare_tracks, fake_vpresults, run_both
 
 pytestmark = pytest.mark.gpu
 
@@ -66,26 +66,10 @@ def test_max_valid_conns_cap():
     compare_tracks(eng, orc)
 
 
-def _fake_vpresults(sc, seed):
-    """Random but well-formed VPResults: ~60% of the lines of every image carry one of 3 VPs."""
-    from limap_b200.vplib import VPResult
-    rng = np.random.default_rng(seed)
-    out = {}
-    for v, i in enumerate(sc.img_ids):
-        L = int(sc.line_off[v + 1] - sc.line_off[v])
-        vps = rng.normal(size=(3, 3))
-        vps[:, :2] *= 1000.0
-        vps /= np.linalg.norm(vps, axis=1, keepdims=True)
-        labels = rng.integers(0, 3, L)
-        labels[rng.random(L) < 0.4] = -1
-        out[int(i)] = VPResult(labels, vps)
-    return out
-
-
 def test_vp_proposals():
     # use_vp: up to three proposals per match row, [vp1, vp2, algebraic] (base_line_triangulator.cc:258-326)
     sc = make_scene(V=6, L=60, N=4, K=3, seed=21)
-    vp = _fake_vpresults(sc, 5)
+    vp = fake_vpresults(sc, 5)
     eng, orc = run_both(sc, _cfg(use_vp=True, debug_mode=True), vpresults=vp)
     st = compare_nodes(sc, eng, orc, debug=True)
     assert st["candidates"] > 1.2 * run_both(sc, _cfg())[0].stats()["n_candidates"]
