@@ -36,10 +36,15 @@ def test_medium_scene_default_yaml():
     assert tr["tracks"] > 100
 
 
-def test_cpp_defaults_and_outer_edge_filter():
-    # C++ defaults differ from the yaml (min_length_2d 20, angle 5, min_num_outer_edges 1, linker thresholds)
+@pytest.mark.parametrize("min_outer", [1, 2, 3])
+def test_cpp_defaults_and_outer_edge_filter(min_outer):
+    # C++ defaults differ from the yaml (min_length_2d 20, angle 5, min_num_outer_edges 1, linker thresholds); 2 and 3
+    # make filterNodeByNumOuterEdges peel further, as dropped nodes cost their parents outer edges
     sc = make_scene(V=8, L=120, N=5, K=5, seed=13)
-    eng, orc = run_both(sc, {})
+    eng, orc = run_both(sc, {"min_num_outer_edges": min_outer})
+    unfiltered, _ = run_both(sc, {"min_num_outer_edges": 0})
+    support = lambda e: int(e.build_tracks()["track_off"][-1])
+    assert support(eng) < support(unfiltered)  # the filter removes nodes from the track graph of this scene
     compare_nodes(sc, eng, orc)
     compare_tracks(eng, orc)
 
@@ -179,7 +184,7 @@ def test_bulk_add_and_pipeline_groups_match_per_image_adds():
         assert sink.tobytes() == nodes_ref.tobytes()
         with pytest.raises(ValueError):
             eng.run(nodes_out=np.zeros(3, NODE_RECORD_DTYPE))
-        # tracks (graph built on the device for min_num_outer_edges = 0; the host-graph path runs in the C++-defaults test)
+        # tracks (min_num_outer_edges = 0; the outer-edge filter runs in the C++-defaults test)
         tr = eng.build_tracks()
         tr_ref = ref.build_tracks()
         for k in ("track_off", "img_ids", "line_ids", "node_ids"):
