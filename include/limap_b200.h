@@ -229,6 +229,38 @@ int64_t lm_remerge_labels(lm_ctx *ctx, int64_t T, const double *track_line, cons
                           const lm_linker_config *linker3d, int32_t *out_labels, int64_t *out_n_edges);
 int lm_merge_get_stats(lm_ctx *ctx, lm_merge_stats *out);
 
+/* ---- fit-and-merge: MergeToLineTracks (merging/merging.cc:347-511) with SetUncertaintySegs3d
+ * (merging_utils.cc:15-25), the merge step of merging.merging (merging.py:6-21) ------------------------------------
+ * Views in ascending image id order: img_ids, model_ids (0 SIMPLE_PINHOLE, 1 PINHOLE), kvec/qvec/tvec as in
+ * lm_scene_upload; line_off[n_views+1]; per line its 2D segment segs[n][4] and 3D fit lines3d[n][6] = start3, end3
+ * (failed fits are zeros: lines of length 0 are no graph node). Neighbours of view v: the image ids
+ * ng_ids[ng_off[v] .. ng_off[v+1]), in the given order, repeats and the image itself allowed. linker2d is used as
+ * given, linker3d under set_to_spatial_merging(). Graph nodes are the non-zero lines in (image, line) order; edges
+ * are numbered in the reference's insertion order. Limits (LM_ERR_INVALID past them, they size the sort keys):
+ * n_views <= 65535, lines per image <= 65535, neighbours per image <= 32767, nodes and edges < 2^31, finite inputs.
+ * Returns the number of tracks (>= 0) or <0; out_counts[3] = graph nodes, graph edges, track supports. */
+typedef struct lm_fit_merge_stats {
+  int64_t n_lines, n_nodes;
+  int64_t n_pairs_tested; /* line pairs the reference's loops hand to check_connection_3d */
+  int64_t n_pairs_gated;  /* of these, pairs past the fp32 gates, decided with the fp64 formulas */
+  int64_t n_edges, n_tracks;
+  int64_t n_retries;      /* reruns of the pair kernel after its edge list overflowed (0 or 1) */
+  double pair_kernel_ms;  /* device time of the pair kernel (last run when retried) */
+  double total_ms;        /* host arrays in to results on the host, wall clock */
+} lm_fit_merge_stats;
+int64_t lm_merge_fits_build(lm_ctx *ctx, int32_t n_views, const int32_t *img_ids, const int32_t *model_ids,
+                            const double *kvec, const double *qvec, const double *tvec, const int64_t *line_off,
+                            const double *segs, const double *lines3d, const int64_t *ng_off, const int32_t *ng_ids,
+                            double var2d, const lm_linker_config *linker2d, const lm_linker_config *linker3d,
+                            int64_t *out_counts);
+/* Results of the last lm_merge_fits_build (sizes from its counts): unc[n] = uncertainty of every line, length[n] =
+ * its Line3d::length() (the support score, bit-exact), node_line[nodes] = global line index (line_off[v] + line) of each graph node, edges[n_edges][2] = (node1, node2)
+ * and sim[n_edges] in insertion order, track_off[T+1], track_nodes[supports] (node order within a track),
+ * track_line[T][7] = start3, end3, uncertainty. Any pointer may be NULL. */
+int lm_merge_fits_get(lm_ctx *ctx, double *unc, double *length, int64_t *node_line, int32_t *edges, double *sim, int64_t *track_off,
+                      int32_t *track_nodes, double *track_line);
+int lm_merge_fits_get_stats(lm_ctx *ctx, lm_fit_merge_stats *out);
+
 /* ---- line refinement / line bundle adjustment (cameras constant) ---------------------------------
  * Replaces HybridBAEngine::{InitLineTracks,SetUp,Solve,GetOutputLineTracks}
  * (optimize/hybrid_bundle_adjustment/hybrid_bundle_adjustment.cc:39-59,156-264,298-310) as called by

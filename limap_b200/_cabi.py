@@ -56,6 +56,11 @@ class MergeStats(C.Structure):
                 ("last_remerge_kernel_ms", C.c_float)]
 
 
+class FitMergeStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("n_lines", "n_nodes", "n_pairs_tested", "n_pairs_gated", "n_edges", "n_tracks",
+                                         "n_retries")] + [("pair_kernel_ms", C.c_double), ("total_ms", C.c_double)]
+
+
 NODE_RECORD_DTYPE = np.dtype([("line", np.float64, 9), ("score", np.float64), ("ng_view", np.int32),
                               ("ng_line", np.int32), ("n_cand", np.int32), ("n_valid", np.int32)])
 
@@ -111,6 +116,9 @@ _SIGS = {
     "lm_aggregate_lines": (C.c_int, [C.c_int64, _P, _P, _P, C.c_int32, _P]),
     "lm_remerge_labels": (C.c_int64, [_P, C.c_int64, _P, _P, _P, _P, _P]),
     "lm_merge_get_stats": (C.c_int, [_P, _P]),
+    "lm_merge_fits_build": (C.c_int64, [_P, C.c_int32] + [_P] * 10 + [C.c_double, _P, _P, _P]),
+    "lm_merge_fits_get": (C.c_int, [_P] * 9),
+    "lm_merge_fits_get_stats": (C.c_int, [_P, _P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS)
 

@@ -650,6 +650,73 @@ class LineTrack:
                 "score_list": list(self.score_list)}
 
 
+class PatchNode:
+    """base/graph.h:37-46 (read-only view of one node of a Graph)."""
+
+    def __init__(self, image_idx, line_idx, node_idx):
+        self.image_idx, self.line_idx, self.node_idx = int(image_idx), int(line_idx), int(node_idx)
+
+
+class Edge:
+    """base/graph.h:25-35 (read-only view of one undirected edge of a Graph)."""
+
+    def __init__(self, node_idx1, node_idx2, sim, edge_idx):
+        self.node_idx1, self.node_idx2, self.sim, self.edge_idx = int(node_idx1), int(node_idx2), float(sim), int(edge_idx)
+
+    @property
+    def similarity(self):
+        return self.sim
+
+
+class Graph:
+    """base/graph.h:48-67 as base/bindings.cc:58-68 exposes it, read-only and backed by arrays: node i is
+    (image_idx[i], line_idx[i]); edge e is (node1[e], node2[e], sim[e]) in insertion order. Node and edge objects are
+    built on access."""
+
+    def __init__(self, image_idx=(), line_idx=(), node1=(), node2=(), sim=()):
+        self.image_idx = np.asarray(image_idx, np.int64)
+        self.line_idx = np.asarray(line_idx, np.int64)
+        self.node1 = np.asarray(node1, np.int64)
+        self.node2 = np.asarray(node2, np.int64)
+        self.sim = np.asarray(sim, np.float64)
+
+    @property
+    def nodes(self):
+        return [PatchNode(i, l, k) for k, (i, l) in enumerate(zip(self.image_idx.tolist(), self.line_idx.tolist()))]
+
+    @property
+    def undirected_edges(self):
+        return [Edge(a, b, w, e) for e, (a, b, w) in enumerate(zip(self.node1.tolist(), self.node2.tolist(),
+                                                                  self.sim.tolist()))]
+
+    @property
+    def node_map(self):
+        return {(i, l): k for k, (i, l) in enumerate(zip(self.image_idx.tolist(), self.line_idx.tolist()))}
+
+    def get_node_id(self, image_idx, line_idx):  # graph.cc:72-78: size_t(-1) when absent
+        return self.node_map.get((int(image_idx), int(line_idx)), 2 ** 64 - 1)
+
+    def _endpoints(self):
+        # AddEdge appends the edge to out_edges and in_edges of both ends (graph.cc:18-21, :80-86)
+        ends = np.empty(2 * len(self.node1), np.int64)
+        ends[0::2], ends[1::2] = self.node1, self.node2
+        return ends
+
+    @property
+    def input_degrees(self):
+        return np.bincount(self._endpoints(), minlength=len(self.image_idx)).tolist()
+
+    @property
+    def output_degrees(self):
+        return self.input_degrees
+
+    @property
+    def scores(self):  # graph.cc:45-55: sum of the out-edge similarities, added in insertion order
+        s = np.zeros(len(self.image_idx))
+        np.add.at(s, self._endpoints(), np.repeat(self.sim, 2))
+        return [(float(x), k) for k, x in enumerate(s.tolist())]
+
+
 class _LinkerConfig:
     _defaults = {}
 

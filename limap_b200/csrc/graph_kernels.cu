@@ -77,9 +77,7 @@ __global__ void edge_order_keys_kernel(const uint64_t *__restrict__ kc, const do
   if (e >= n2) return;
   const uint64_t i0 = (uint32_t)gidx[kc[e] >> 32], i1 = (uint32_t)gidx[kc[e] & 0xffffffffull];
   by_nodes[e] = ~(i0 << 32 | i1);
-  uint64_t b = (uint64_t)__double_as_longlong(wc[e]);
-  b = (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-  by_score[e] = ~b;
+  by_score[e] = descending_double_key(wc[e]);
 }
 
 void launch_undirected_keys(const int64_t *edges, int64_t ne, uint64_t *keys, cudaStream_t s) {

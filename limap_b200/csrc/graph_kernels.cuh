@@ -7,6 +7,13 @@
 
 namespace lm {
 
+// Radix key that sorts finite doubles in descending order (ascending order of the complemented, sign-folded bits).
+__device__ __forceinline__ uint64_t descending_double_key(double w) {
+  uint64_t b = (uint64_t)__double_as_longlong(w);
+  b = (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+  return ~b;
+}
+
 void launch_undirected_keys(const int64_t *edges, int64_t ne, uint64_t *keys, cudaStream_t s);
 void launch_keys_to_pairs(const uint64_t *keys, int64_t n, int64_t *pairs, cudaStream_t s);
 void launch_nonzero_flags(const double *w, int64_t n, uint32_t *flag, cudaStream_t s);

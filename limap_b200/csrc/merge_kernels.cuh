@@ -37,4 +37,46 @@ void launch_remerge_dirs(const double *lines, int64_t T, const double origin[3],
                          float4 *ballf, cudaStream_t s);
 void launch_remerge_pairs(const RemergeParams &p, cudaStream_t s);
 
+// MergeToLineTracks from per-image 3D fits (merging/merging.cc:347-511).
+struct FitView {       // CameraView as Line3d::projection / computeUncertainty evaluate it
+  double R[9], t[3];   // row-major rotation, translation
+  double fx, fy, cx, cy, f; // f = Camera::uncertainty's focal length
+};
+struct FitPrepParams {
+  const FitView *views;      // [V]
+  const int64_t *line_off;   // [V+1]
+  const double *lines3d;     // [n][6]
+  int32_t V;
+  int64_t n;
+  double var2d, ox, oy, oz, th_innerseg;
+  double *rec;               // [n][7] start, end, uncertainty
+  double *len;               // [n] Line3d::length(), bit-exact
+  uint8_t *nonzero;          // [n] length != 0: the line is a graph node
+  float4 *dirf, *ballf;      // [n] gate records
+};
+void launch_fit_prep(const FitPrepParams &p, cudaStream_t s);
+
+struct FitTile { int32_t va, vb, slot, tiles; }; // slot < 0: self block of va; tiles = ta << 16 | tb
+struct FitPairParams {
+  const FitView *views;
+  const int64_t *line_off;
+  const int32_t *img_ids;
+  const double4 *segs;       // [n]
+  const double *rec;         // [n][7]
+  const uint8_t *nonzero;
+  const float4 *dirf, *ballf;
+  const FitTile *tiles;
+  LinkerDev<double> lk3, lk2; // lk3 after set_to_spatial_merging()
+  float cos_gate;
+  int use_gate, use_ball;
+  unsigned long long *keys;  // [capacity] insertion key
+  unsigned long long *pairs; // [capacity] line1 << 32 | line2 (global line indices; node ids keep their order)
+  unsigned long long *counter; // [3]: edges, pairs past the gates, pairs tested
+  unsigned long long capacity;
+};
+void launch_fit_pairs(const FitPairParams &p, int64_t n_tiles, cudaStream_t s);
+// keys of the greedy order (descending (sim, node1, node2)) of the edges in insertion order; sim[e] = len1 + len2
+void launch_fit_order_keys(const unsigned long long *pairs, const double *len, int64_t n,
+                           unsigned long long *by_nodes, unsigned long long *by_score, double *sim, cudaStream_t s);
+
 } // namespace lm

@@ -277,8 +277,8 @@ class BAEngine:
 
 
 class MergeEngine:
-    """Track filters and remerge on flat arrays (include/limap_b200.h: lm_tracks_support_flags,
-    lm_remerge_labels, lm_aggregate_lines)."""
+    """Track filters, remerge and the fit-and-merge track build on flat arrays (include/limap_b200.h:
+    lm_tracks_support_flags, lm_remerge_labels, lm_aggregate_lines, lm_merge_fits_build)."""
 
     def __init__(self, device=0, ctx=None):
         self.ctx = ctx if ctx is not None else Context(device)
@@ -309,6 +309,32 @@ class MergeEngine:
         ng = check(lib().lm_remerge_labels(self.ctx.handle, T, ptr(track_line), ptr(active), C.byref(linker3d),
                                            ptr(labels), C.byref(ne)))
         return labels, int(ng), int(ne.value)
+
+    def merge_fits(self, img_ids, model_ids, kvec, qvec, tvec, line_off, segs, lines3d, ng_off, ng_ids, var2d,
+                   linker2d, linker3d):
+        """MergeToLineTracks on flat arrays (lm_merge_fits_build); linker2d / linker3d: config.LinkerConfig. Returns
+        dict(unc, length, node_line, edges, sim, track_off, track_nodes, track_line)."""
+        i32 = lambda a: np.ascontiguousarray(a, np.int32)
+        i64 = lambda a: np.ascontiguousarray(a, np.int64)
+        f64 = lambda a: np.ascontiguousarray(a, np.float64)
+        segs = np.asarray(segs, np.float64).reshape(-1, np.shape(segs)[-1] if np.size(segs) else 4)[:, :4]
+        a = [i32(img_ids), i32(model_ids), f64(kvec), f64(qvec), f64(tvec), i64(line_off), f64(segs),
+             f64(lines3d).reshape(-1, 6), i64(ng_off), i32(ng_ids)]
+        counts = np.zeros(3, np.int64)
+        T = check(lib().lm_merge_fits_build(self.ctx.handle, len(a[0]), *[ptr(x) for x in a], float(var2d),
+                                            C.byref(linker2d), C.byref(linker3d), ptr(counts)))
+        nn, ne, ns = (int(x) for x in counts)
+        out = dict(unc=np.zeros(int(a[5][-1])), length=np.zeros(int(a[5][-1])), node_line=np.zeros(nn, np.int64), edges=np.zeros((ne, 2), np.int32),
+                   sim=np.zeros(ne), track_off=np.zeros(T + 1, np.int64), track_nodes=np.zeros(ns, np.int32),
+                   track_line=np.zeros((T, 7)))
+        check(lib().lm_merge_fits_get(self.ctx.handle, *[ptr(out[k]) for k in (
+            "unc", "length", "node_line", "edges", "sim", "track_off", "track_nodes", "track_line")]))
+        return out
+
+    def fit_merge_stats(self):
+        st = _cabi.FitMergeStats()
+        check(lib().lm_merge_fits_get_stats(self.ctx.handle, C.byref(st)))
+        return {k: getattr(st, k) for k, _ in _cabi.FitMergeStats._fields_}
 
     @staticmethod
     def aggregate(off, lines, scores, num_outliers):

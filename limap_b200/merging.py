@@ -4,13 +4,14 @@ Mirrors src/limap/merging/merging.py:24-83 (remerge, check_track_by_reprojection
 filter_tracks_by_reprojection, check_sensitivity, filter_tracks_by_sensitivity, filter_tracks_by_overlap) over
 merging/merging_utils.cc:27-155 and merging/merging.cc:513-645. The per-support geometry and the O(T^2)
 pair test run on the GPU (include/limap_b200.h); list surgery on LineTrack objects stays in Python like the
-reference's std::vector code. `merging()` (MergeToLineTracks from per-image 3D segments, merging.py:6-21) is
-the fitnmerge front end and outside the hot path (SURVEY.md §8).
+reference's std::vector code. `merging()` (MergeToLineTracks from per-image 3D segments, merging.py:6-21,
+merging.cc:347-511), the merge step of the fit-and-merge pipeline, runs its O(lines^2 x neighbours) pair tests,
+edge sorts and uncertainties on the GPU (lm_merge_fits_build); the union-find and the aggregation run on the host.
 """
 import numpy as np
 
 from . import base
-from .config import LINKER3D_DEFAULTS, make_linker
+from .config import LINKER2D_DEFAULTS, LINKER3D_DEFAULTS, make_linker
 from .engine import MergeEngine
 
 _engine = None
@@ -21,6 +22,80 @@ def _eng():
     if _engine is None:
         _engine = MergeEngine()
     return _engine
+
+
+def _SetUncertaintySegs3d(lines, view, var2d):
+    """merging_utils.cc:15-25: copies of the 3D lines with uncertainty = Line3d::computeUncertainty(view, var2d)."""
+    out = []
+    for l in lines:
+        n = base.Line3d(l.start, l.end, l.score, l.depths[0], l.depths[1], l.uncertainty)
+        n.set_uncertainty(n.computeUncertainty(view, var2d))
+        out.append(n)
+    return out
+
+
+def _linker_cfg(cfg, defaults):
+    d = cfg.as_dict() if hasattr(cfg, "as_dict") else dict(cfg or {})
+    return make_linker(defaults, d)
+
+
+def merging(linker, all_2d_segs, imagecols, seg3d_list, neighbors, var2d=5.0):
+    """merging.py:6-21: SetUncertaintySegs3d per image, then MergeToLineTracks (merging.cc:347-511) on the GPU.
+    linker: base.LineLinker; all_2d_segs[img_id]: (N, 4|5) segments; seg3d_list[img_id]: N (2, 3) fits, zeros where the
+    fit failed; neighbors: {img_id: [img_id, ...]}. Returns (base.Graph, list of base.LineTrack)."""
+    ids = imagecols.get_img_ids()
+    if len(neighbors) != len(ids):  # THROW_CHECK_EQ(all_lines_2d.size(), neighbors.size())
+        raise RuntimeError(f"Check failed: all_lines_2d.size() == neighbors.size() ({len(ids)} vs. {len(neighbors)})")
+    segs, fits, line_off = [], [], [0]
+    for img_id in ids:
+        s2 = np.asarray(all_2d_segs[img_id], np.float64)
+        if s2.ndim != 2 or (s2.shape[0] != 0 and s2.shape[1] < 4):
+            raise RuntimeError("THROW_CHECK_GE(segs2d.cols(), 4)")
+        f3 = np.asarray(seg3d_list[img_id], np.float64).reshape(-1, 2, 3)
+        if len(f3) != len(s2):  # THROW_CHECK_EQ(all_lines_2d.at(image_id).size(), all_lines_3d.at(image_id).size())
+            raise RuntimeError(f"Check failed: 2D lines ({len(s2)}) and 3D lines ({len(f3)}) of image {img_id} differ")
+        segs.append(s2[:, :4].reshape(-1, 4))
+        fits.append(f3)
+        line_off.append(line_off[-1] + len(s2))
+    ng_off, ng_ids = [0], []
+    for img_id in ids:
+        if img_id not in neighbors:
+            raise IndexError("map::at")  # neighbors.at(image_id)
+        for j in neighbors[img_id]:
+            if not imagecols.exist_image(int(j)):
+                raise IndexError("map::at")  # all_lines_2d.at(ng_image_id)
+            ng_ids.append(int(j))
+        ng_off.append(len(ng_ids))
+    l2 = _linker_cfg(linker.linker_2d.config, LINKER2D_DEFAULTS)
+    l3 = _linker_cfg(linker.linker_3d.config, LINKER3D_DEFAULTS)
+    img_ids, model, kvec, qvec, tvec = imagecols.arrays()
+    r = _eng().merge_fits(img_ids, model, kvec, qvec, tvec, np.asarray(line_off, np.int64),
+                          np.concatenate(segs) if segs else np.zeros((0, 4)),
+                          np.concatenate(fits) if fits else np.zeros((0, 2, 3)),
+                          np.asarray(ng_off, np.int64), np.asarray(ng_ids, np.int32), var2d, l2, l3)
+    line_off = np.asarray(line_off, np.int64)
+    view = np.searchsorted(line_off, r["node_line"], side="right") - 1
+    node_img = np.asarray(ids, np.int64)[view] if len(view) else np.zeros(0, np.int64)
+    node_lid = r["node_line"] - line_off[view] if len(view) else np.zeros(0, np.int64)
+    graph = base.Graph(node_img, node_lid, r["edges"][:, 0], r["edges"][:, 1], r["sim"])
+    flat_segs = np.concatenate(segs) if segs else np.zeros((0, 4))
+    flat_fits = np.concatenate(fits) if fits else np.zeros((0, 2, 3))
+    tracks = []
+    for t in range(len(r["track_off"]) - 1):
+        tr = base.LineTrack()
+        for k in r["track_nodes"][r["track_off"][t]:r["track_off"][t + 1]].tolist():
+            g = int(r["node_line"][k])
+            l3d = base.Line3d(flat_fits[g, 0], flat_fits[g, 1], uncertainty=r["unc"][g])
+            tr.node_id_list.append(k)
+            tr.image_id_list.append(int(node_img[k]))
+            tr.line_id_list.append(int(node_lid[k]))
+            tr.line2d_list.append(base.Line2d(flat_segs[g, :2], flat_segs[g, 2:4]))
+            tr.line3d_list.append(l3d)
+            tr.score_list.append(float(r["length"][g]))  # Line3d::length() (merging.cc:493)
+        tl = r["track_line"][t]
+        tr.line = base.Line3d(tl[:3], tl[3:6], uncertainty=tl[6])
+        tracks.append(tr)
+    return graph, tracks
 
 
 def _flatten(linetracks, imagecols):

@@ -257,6 +257,80 @@ CONFIGS = {
 
 
 @dataclass
+class FitScene:
+    """Per-image 3D fits of every 2D segment of a Scene (the input of merging.merging, merging.py:6-21): lines3d[n,2,3]
+    in the scene's flat segment order, zeros where the fit failed; neighbours as ng_ids[ng_off[v] .. ng_off[v+1])."""
+    img_ids: np.ndarray
+    model_ids: np.ndarray
+    kvec: np.ndarray
+    qvec: np.ndarray
+    tvec: np.ndarray
+    line_off: np.ndarray
+    segs: np.ndarray
+    lines3d: np.ndarray
+    neighbors: dict
+    ng_off: np.ndarray = None
+    ng_ids: np.ndarray = None
+
+    def __post_init__(self):
+        self.set_neighbors(self.neighbors)
+
+    def set_neighbors(self, neighbors):
+        self.neighbors = {int(k): [int(x) for x in v] for k, v in neighbors.items()}
+        lists = [self.neighbors.get(int(i), []) for i in self.img_ids]
+        self.ng_off = np.concatenate([[0], np.cumsum([len(x) for x in lists])]).astype(np.int64)
+        self.ng_ids = np.asarray([x for lst in lists for x in lst], np.int32)
+
+    def segs_of(self, view):
+        return self.segs[self.line_off[view]:self.line_off[view + 1]]
+
+    def fits_of(self, view):
+        return self.lines3d[self.line_off[view]:self.line_off[view + 1]]
+
+
+def make_fits(scene, depth_noise=1e-3, fail_frac=0.1, seed=0, degenerate_frac=0.01):
+    """What line fitting from depth (runners/line_fitnmerge.py:30-56) would give on `scene`: each endpoint of a segment
+    of a GT line is back-projected onto that line (the point of the line closest to the endpoint's ray), then moved along
+    the ray by a relative depth error N(0, depth_noise). Clutter and a `fail_frac` share of the segments get zero fits
+    (failed fits, line_fitnmerge.py:52-55); a `degenerate_frac` share gets start == end != 0."""
+    from .base import _quat_to_R
+    rng = np.random.default_rng(seed)
+    n = len(scene.segs)
+    lines3d = np.zeros((n, 2, 3))
+    for v in range(len(scene.img_ids)):
+        R = _quat_to_R(scene.qvec[v])
+        t = scene.tvec[v]
+        C = -R.T @ t
+        fx, fy, cx, cy = scene.kvec[v]
+        if scene.model_ids[v] == 0:
+            fy = fx
+        for g in range(int(scene.line_off[v]), int(scene.line_off[v + 1])):
+            gid = int(scene.gt_id[g])
+            if gid < 0:
+                continue
+            P0, P1 = scene.gt_lines[gid, :3], scene.gt_lines[gid, 3:]
+            u = (P1 - P0) / np.linalg.norm(P1 - P0)
+            for k in range(2):
+                x, y = scene.segs[g, 2 * k:2 * k + 2]
+                r = R.T @ np.array([(x - cx) / fx, (y - cy) / fy, 1.0])
+                r /= np.linalg.norm(r)
+                # closest points of the ray C + s r and the line P0 + w u
+                w0 = C - P0
+                b, d, e = r @ u, r @ w0, u @ w0
+                den = 1.0 - b * b
+                s = (b * e - d) / den if den > 1e-12 else -d
+                lines3d[g, k] = C + r * s * (1.0 + depth_noise * rng.normal())
+    fail = rng.random(n) < fail_frac
+    lines3d[fail] = 0.0
+    nz = np.flatnonzero(np.abs(lines3d).sum(axis=(1, 2)) > 0)
+    degen = nz[rng.random(len(nz)) < degenerate_frac]
+    lines3d[degen, 1] = lines3d[degen, 0]
+    return FitScene(img_ids=scene.img_ids.copy(), model_ids=scene.model_ids.copy(), kvec=scene.kvec.copy(),
+                    qvec=scene.qvec.copy(), tvec=scene.tvec.copy(), line_off=scene.line_off.copy(),
+                    segs=scene.segs.copy(), lines3d=lines3d, neighbors=dict(scene.neighbors))
+
+
+@dataclass
 class TrackSet:
     """Flat line tracks for the refinement path (BASELINE.json configs[3]): sup_off[T+1]; per support:
     2D segment, camera (kvec,qvec,tvec), image id and the per-node 3D line (track.line3d_list)."""
