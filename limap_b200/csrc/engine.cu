@@ -733,11 +733,15 @@ int lm_tri_run(lm_ctx *c) {
     c->outside_shard_clean = true;
   }
   // The staging capacity of the node kernel (candidates per node held in shared memory) comes from the previous run
-  // (default: what four CTAs per SM allow); the kernel flags nodes that do not fit and the run is repeated once with
+  // (default: 224); the kernel flags nodes that do not fit and the run is repeated once with
   // the exact size. No read-back, no host synchronisation until everything of this run is queued.
   const bool fast_kernel = p.fast_forms && !p.use_endpoints_triangulation;
   const size_t smem_limit = (size_t)std::max(0, c->max_smem_optin - 1024);
-  int cap = c->cap_hint > 0 ? c->cap_hint : 224;
+  // capacities are multiples of 32 for the generic layout (its start-point prefilter pads a node's candidates to a
+  // multiple of 32) and of 8 for the fast one (hypersim100's 200-row nodes fit at cap 200, five CTAs per SM)
+  const int cap_step = fast_kernel ? 8 : 32;
+  auto round_cap = [&](int64_t n) { return (int)std::max<int64_t>(cap_step, (n + cap_step - 1) / cap_step * cap_step); };
+  int cap = c->cap_hint > 0 ? round_cap(c->cap_hint) : 224;
   if (exhaustive && c->cap_hint == 0) { // every node sees all lines of every neighbour: known on the host
     int64_t mr = 0, cur = 0;
     int cur_src = -1;
@@ -747,8 +751,7 @@ int lm_tri_run(lm_ctx *c) {
       mr = std::max(mr, cur);
     }
     if (mr * ns > 65535) return fail(LM_ERR_INVALID, "more than 65535 candidates possible for one 2D line");
-    cap = 32;
-    while (cap < mr * ns) cap += 32;
+    cap = round_cap(mr * ns);
   }
   while ((int)c->evk.size() < 2 * n_groups) {
     cudaEvent_t e;
@@ -885,9 +888,7 @@ int lm_tri_run(lm_ctx *c) {
   int max_rows_all = 0;
   for (int g = 0; g < n_groups; ++g) max_rows_all = std::max(max_rows_all, (int)hs[16 + g]);
   if ((int64_t)max_rows_all * ns > 65535) return fail(LM_ERR_INVALID, "more than 65535 candidates possible for one 2D line");
-  int need_cap = 32;
-  while (need_cap < max_rows_all * ns) need_cap += 32;
-  c->cap_hint = need_cap;
+  c->cap_hint = round_cap((int64_t)max_rows_all * ns);
   if (hs[2] != 0) { // some node did not fit the staging area sized from the hint: repeat with the exact size
     if (c->run_retry) { c->run_retry = 0; return fail(LM_ERR_STATE, "node staging overflow after resizing"); }
     c->run_retry = 1;

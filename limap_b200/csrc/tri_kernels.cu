@@ -18,8 +18,11 @@
 
 namespace lm {
 
+// CTAs per SM the registers of the headline instantiation tri_node_kernel<false, false, true> are sized for (5: 96
+// registers, with the fast staging layout at cap 200 in 42.8 KB of shared memory); the slab, VP and generic
+// instantiations stay at 4 (128 registers)
 #ifndef LM_TRI_MIN_BLOCKS
-#define LM_TRI_MIN_BLOCKS 4
+#define LM_TRI_MIN_BLOCKS 5
 #endif
 static constexpr int kThreads = 128;
 static constexpr int kWarps = kThreads / 32;
@@ -44,11 +47,12 @@ static constexpr int kListExtra = kFlush + 32;
 static constexpr int kCandBytes = 17 * 8 + 48 + 8;
 
 // Shared-memory staging per node. Generic layout: 17 doubles + 48-byte fp32 gate record + ng/row per candidate, two
-// survivor lists and one prefilter list per warp. Fast layout (reduced-form scorer, plane-pair triangulation): 20 doubles
-// (three reciprocals more), a 32-byte gate record, ng/row, the depth-sorted order (float key + uint16 index) per
-// candidate, and per warp one pair list (uint16) with its scores (double): 246 bytes per candidate slot.
+// survivor lists and one prefilter list per warp. Fast layout (reduced-form scorer, plane-pair triangulation): 16 doubles
+// (three reciprocals more, and not the matched 2D segment, which the scorer reloads through ng), a 32-byte gate record,
+// ng/row, the depth-sorted order (float key + uint16 index) per candidate, and per warp one pair list (uint16) with its
+// scores (double): 214 bytes per candidate slot, 42.8 KB at cap 200, which lets five CTAs share an SM.
 size_t tri_smem_bytes(int cap, bool fast) {
-  if (fast) return (size_t)cap * (20 * 8 + kWarps * 8 + 32 + 8 + 4 + 2 + kWarps * 2);
+  if (fast) return (size_t)cap * (16 * 8 + kWarps * 8 + 32 + 8 + 4 + 2 + kWarps * 2);
   return (size_t)cap * kCandBytes + (size_t)kWarps * 2 * (cap + kListExtra) * 4 + (size_t)kWarps * cap * 2;
 }
 
@@ -73,7 +77,7 @@ struct __align__(16) GateRecF {
 
 struct Slab {
   double *sx, *sy, *sz, *ex, *ey, *ez, *dx, *dy, *dz, *zs, *ze, *unc, *q0, *q1, *q2, *q3, *score;
-  double *izs2, *ize2, *inb; // fast layout only: 1/(zs+EPS)^2, 1/(ze+EPS)^2, 1/|q|^2
+  double *izs2, *ize2, *inb; // fast layout only: 1/(zs+EPS)^2, 1/(ze+EPS)^2, 1/|q|^2 (q0..q3: generic layout only)
   GateRec *gate;
   uint32_t *ng, *row;
   uint32_t *list;            // [kWarps][2][cap + kListExtra]: (row << 16 | j) survivor entries
@@ -100,20 +104,20 @@ struct Slab {
     list = row + cap;
     list0 = reinterpret_cast<uint16_t *>(list + (size_t)kWarps * (fast ? 1 : 2) * (cap + kListExtra));
   }
+  // cap is a multiple of 8: gatef and the staged views of the VP instantiation (psc + 4 cap) stay 16-byte aligned
   LM_D void carve_fast(char *base, int cap) {
     double *d = reinterpret_cast<double *>(base);
     sx = d; sy = sx + cap; sz = sy + cap; ex = sz + cap; ey = ex + cap; ez = ey + cap;
     dx = ez + cap; dy = dx + cap; dz = dy + cap; zs = dz + cap; ze = zs + cap; unc = ze + cap;
-    q0 = unc + cap; q1 = q0 + cap; q2 = q1 + cap; q3 = q2 + cap; score = q3 + cap;
-    izs2 = score + cap; ize2 = izs2 + cap; inb = ize2 + cap;
-    psc = inb + cap;                                              // byte 160 cap
-    gatef = reinterpret_cast<GateRecF *>(psc + (size_t)kWarps * cap); // byte 192 cap
-    ng = reinterpret_cast<uint32_t *>(gatef + cap);               // byte 224 cap
+    score = unc + cap; izs2 = score + cap; ize2 = izs2 + cap; inb = ize2 + cap;
+    psc = inb + cap;                                              // byte 128 cap
+    gatef = reinterpret_cast<GateRecF *>(psc + (size_t)kWarps * cap); // byte 160 cap
+    ng = reinterpret_cast<uint32_t *>(gatef + cap);               // byte 192 cap
     row = ng + cap;
-    slam = reinterpret_cast<float *>(row + cap);                  // byte 232 cap
-    sidx = reinterpret_cast<uint16_t *>(slam + cap);              // byte 236 cap
-    pent = sidx + cap;                                            // byte 238 cap, [kWarps][cap]
-    gate = nullptr; list = nullptr; list0 = nullptr;
+    slam = reinterpret_cast<float *>(row + cap);                  // byte 200 cap
+    sidx = reinterpret_cast<uint16_t *>(slam + cap);              // byte 204 cap
+    pent = sidx + cap;                                            // byte 206 cap, [kWarps][cap]
+    q0 = q1 = q2 = q3 = nullptr; gate = nullptr; list = nullptr; list0 = nullptr;
   }
 };
 
@@ -175,7 +179,7 @@ LM_D bool triangulate_point(const ViewD &v1, const ViewD &v2, vec3<double> n1e, 
   return !(z1 < consts<double>::eps() || z2 < consts<double>::eps());
 }
 
-// Per-node constants of the source line (computed redundantly by every thread: ~60 flops).
+// Per-node constants of the source line (computed by one thread into shared memory: ~60 flops).
 struct Src {
   double4 l1;
   vec3<double> w1s, w1e;     // M1 [p;1] (unnormalised world rays)
@@ -457,8 +461,10 @@ LM_D double angle2_deg(double t, double abs_cos) {
 // Reduced-form pair score: same value as pair_score() up to rounding. min over sub-scores of exp(-(v/sigma)^2/2)
 // == exp(-max (v/sigma)^2 / 2), so the squared normalised deviations are maximised and one exponential is taken;
 // angles come from sin^2 (cross products) through the asin^2 series, distances stay squared, and the divisors
-// that depend on one candidate only (depths of l_i, |q_j|^2) are reciprocals prepared in phase A.
-LM_D double pair_score_fast(const TriParams &p, const Slab &sl, int i, int j, uint32_t vj) {
+// that depend on one candidate only (depths of l_i, |q_j|^2) are reciprocals prepared in phase A. The 2D segment q_j is
+// read through ng_j from the segment table (L1/L2-resident) rather than staged per candidate.
+LM_D double pair_score_fast(const TriParams &p, const Slab &sl, int i, int j, uint32_t ngj) {
+  const uint32_t vj = ngj >> 16;
   const double EPS = consts<double>::eps();
   const LinkerDev<double> &c3 = p.l3d;
   const LinkerDev<double> &c2 = p.l2d;
@@ -484,7 +490,8 @@ LM_D double pair_score_fast(const TriParams &p, const Slab &sl, int i, int j, ui
   const vec3<double> hs = proj_h(v.P, si), he = proj_h(v.P, ei);
   const double ws = 1.0 / (hs.z + EPS), we = 1.0 / (he.z + EPS);
   const vec2<double> as = mk2(hs.x * ws, hs.y * ws), ae = mk2(he.x * we, he.y * we);
-  const vec2<double> bs = mk2(sl.q0[j], sl.q1[j]), be = mk2(sl.q2[j], sl.q3[j]);
+  const double4 q = ld_seg(&p.segs[p.line_off[vj] + (ngj & 0xffffu)]);
+  const vec2<double> bs = mk2(q.x, q.y), be = mk2(q.z, q.w);
   const vec2<double> va = ae - as, vb = be - bs;
   const double na2 = dot(va, va), nb2 = dot(vb, vb);
   const double dab = dot(va, vb);
@@ -608,12 +615,14 @@ LM_D bool gate2d(const TriParams &p, const seg<vec3<double>> &Li, const Slab &sl
 // instantiation keeps the reference-structured scorer, the 2d margin gates and endpoint triangulation. Splitting
 // them keeps the hot kernel's code (and instruction-cache footprint) small.
 template <bool SLAB, bool VP, bool FAST>
-__global__ void __launch_bounds__(kThreads, LM_TRI_MIN_BLOCKS) tri_node_kernel(const __grid_constant__ TriParams p) {
+__global__ void __launch_bounds__(kThreads, (!SLAB && !VP && FAST) ? LM_TRI_MIN_BLOCKS : 4)
+    tri_node_kernel(const __grid_constant__ TriParams p) {
   constexpr int NS = VP ? 3 : 1; // proposal slots per match row: [vp1, vp2, algebraic] (base_line_triangulator.cc:258-326)
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ int s_wtot[kWarps];
   __shared__ int s_nvalid;
   __shared__ int s_next_row;
+  __shared__ Src s_src; // per-node constants of the source line: held in registers they spill in phase A
   __shared__ __align__(8) unsigned long long s_mbar; // completion of the neighbour-view bulk copies of a node
   uint32_t mbar_parity = 0;
   if constexpr (FAST && !SLAB && (LM_TRI_TMA || VP)) {
@@ -689,9 +698,9 @@ __global__ void __launch_bounds__(kThreads, LM_TRI_MIN_BLOCKS) tri_node_kernel(c
     }
     const uint32_t v1i = p.node_view[node];
     const ViewD &v1 = p.views[v1i];
-    Src src;
-    src.l1 = ld_seg(&p.segs[node]);
-    {
+    if (tid == 0) {
+      Src src;
+      src.l1 = ld_seg(&p.segs[node]);
       double dx = src.l1.x - src.l1.z, dy = src.l1.y - src.l1.w;
       src.ok = !(sqrt(dx * dx + dy * dy) <= p.min_length_2d); // :166
       src.w1s = mat3_mul_h(v1.M, src.l1.x, src.l1.y);
@@ -700,7 +709,10 @@ __global__ void __launch_bounds__(kThreads, LM_TRI_MIN_BLOCKS) tri_node_kernel(c
       src.ray1e = normalized(src.w1e);
       src.C1 = mk3(v1.C[0], v1.C[1], v1.C[2]);
       src.n1 = normalized(cross(src.w1s, src.w1e));
+      s_src = src;
     }
+    __syncthreads();
+    const Src &src = s_src;
     if constexpr (FAST && !SLAB && (LM_TRI_TMA || VP)) {
       mbar_wait(&s_mbar, mbar_parity);
       mbar_parity ^= 1u;
@@ -755,6 +767,10 @@ __global__ void __launch_bounds__(kThreads, LM_TRI_MIN_BLOCKS) tri_node_kernel(c
         if (r < nrows) p.row_state[(int64_t)(r0 + r) * NS + k] = 0;
         cnt += oks[k];
       }
+      // the fast layout keeps only 1/|q|^2 of the matched segment: with |q|^2 taken before the barrier, l2 is dead
+      // across it
+      const double qx = l2.z - l2.x, qy = l2.w - l2.y;
+      const double nq2 = qx * qx + qy * qy;
       // stable compaction: exclusive prefix of the per-row candidate counts
       int incl = cnt;
 #pragma unroll
@@ -782,11 +798,11 @@ __global__ void __launch_bounds__(kThreads, LM_TRI_MIN_BLOCKS) tri_node_kernel(c
         sl.ex[idx] = c.e.x; sl.ey[idx] = c.e.y; sl.ez[idx] = c.e.z;
         sl.dx[idx] = d.x; sl.dy[idx] = d.y; sl.dz[idx] = d.z;
         sl.zs[idx] = c.zs; sl.ze[idx] = c.ze; sl.unc[idx] = c.unc;
-        sl.q0[idx] = l2.x; sl.q1[idx] = l2.y; sl.q2[idx] = l2.z; sl.q3[idx] = l2.w;
         if (FAST) {
           const double zs1 = c.zs + consts<double>::eps(), ze1 = c.ze + consts<double>::eps();
-          const double qx = l2.z - l2.x, qy = l2.w - l2.y;
-          sl.izs2[idx] = 1.0 / (zs1 * zs1); sl.ize2[idx] = 1.0 / (ze1 * ze1); sl.inb[idx] = 1.0 / (qx * qx + qy * qy);
+          sl.izs2[idx] = 1.0 / (zs1 * zs1); sl.ize2[idx] = 1.0 / (ze1 * ze1); sl.inb[idx] = 1.0 / nq2;
+        } else {
+          sl.q0[idx] = l2.x; sl.q1[idx] = l2.y; sl.q2[idx] = l2.z; sl.q3[idx] = l2.w;
         }
         sl.ng[idx] = ng;
         sl.row[idx] = (uint32_t)r * NS + k;
@@ -974,7 +990,7 @@ __global__ void __launch_bounds__(kThreads, LM_TRI_MIN_BLOCKS) tri_node_kernel(c
             }
             if (f < fill) {
               const int j = pent[f];
-              psc[f] = pair_score_fast(p, sl, g0 + r, j, (uint32_t)sl.gatef[j].img);
+              psc[f] = pair_score_fast(p, sl, g0 + r, j, sl.ng[j]);
             }
           }
           n2_total += (unsigned long long)fill;
@@ -1093,7 +1109,7 @@ __global__ void __launch_bounds__(kThreads, LM_TRI_MIN_BLOCKS) tri_node_kernel(c
           const uint32_t vj = sl.ng[j] >> 16;
           row = (uint32_t)i;
           key = (row << 16) | vj;
-          if (FAST) sc = pair_score_fast(p, sl, i, j, vj);
+          if (FAST) sc = pair_score_fast(p, sl, i, j, sl.ng[j]);
           else {
             seg<vec3<double>> Li;
             Li.s = mk3(sl.sx[i], sl.sy[i], sl.sz[i]);
@@ -1216,6 +1232,11 @@ template <bool VP, bool FAST> static cudaError_t launch_tri_vf(const TriParams &
   // the opt-in is per device (and per function): set it on every launch above the default limit
   if (smem > 48 * 1024) {
     const cudaError_t e = cudaFuncSetAttribute(tri_node_kernel<false, VP, FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  if constexpr (!VP && FAST) { // five CTAs of 43 KB need the largest shared-memory carveout (228 KB on an H100)
+    const cudaError_t e = cudaFuncSetAttribute(tri_node_kernel<false, VP, FAST>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                               (int)cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return e;
   }
   tri_node_kernel<false, VP, FAST><<<grid, kThreads, smem, s>>>(p);
