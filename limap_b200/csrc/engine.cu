@@ -735,11 +735,9 @@ int lm_tri_run(lm_ctx *c) {
   // The staging capacity of the node kernel (candidates per node held in shared memory) comes from the previous run
   // (default: 224); the kernel flags nodes that do not fit and the run is repeated once with
   // the exact size. No read-back, no host synchronisation until everything of this run is queued.
-  const bool fast_kernel = p.fast_forms && !p.use_endpoints_triangulation;
+  const bool fast_kernel = lm::tri_fast(p);
   const size_t smem_limit = (size_t)std::max(0, c->max_smem_optin - 1024);
-  // capacities are multiples of 32 for the generic layout (its start-point prefilter pads a node's candidates to a
-  // multiple of 32) and of 8 for the fast one (hypersim100's 200-row nodes fit at cap 200, five CTAs per SM)
-  const int cap_step = fast_kernel ? 8 : 32;
+  const int cap_step = lm::tri_cap_step(fast_kernel);
   auto round_cap = [&](int64_t n) { return (int)std::max<int64_t>(cap_step, (n + cap_step - 1) / cap_step * cap_step); };
   int cap = c->cap_hint > 0 ? round_cap(c->cap_hint) : 224;
   if (exhaustive && c->cap_hint == 0) { // every node sees all lines of every neighbour: known on the host
@@ -839,7 +837,7 @@ int lm_tri_run(lm_ctx *c) {
     }
     if (n_group_nodes > 0) {
       CU(cudaEventRecord(c->evk[2 * g], s));
-      CU(lm::launch_tri_node_kernel(p, grid, 128, smem, s));
+      CU(lm::launch_tri_node_kernel(p, grid, smem, s));
       CU(cudaEventRecord(c->evk[2 * g + 1], s));
       group_has_kernel[g] = 1;
       ++launches;

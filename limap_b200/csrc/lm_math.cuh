@@ -19,6 +19,17 @@ inline int current_device_sms() {
   return n;
 }
 
+// Largest i in [0, n) with off[i] <= x, for ascending off with off[0] <= x (0 when n <= 1). The index type I is that
+// of n. LDG: load off through the read-only data cache.
+template <bool LDG = false, typename I, typename T, typename X> LM_D I last_le(const T *off, I n, X x) {
+  I lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const I mid = (lo + hi) >> 1;
+    if ((LDG ? __ldg(&off[mid]) : off[mid]) <= x) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 template <typename T> struct consts;
 template <> struct consts<double> {
   static LM_HD double eps() { return 1e-12; } // util/types.h:34

@@ -53,7 +53,7 @@ LM_D bool linker_check(const LinkerDev<double> &c, const seg<V> &l1, const seg<V
 __global__ void __launch_bounds__(256) support_flags_kernel(const __grid_constant__ SupportParams p) {
   const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= p.S) return;
-  // track of this support: last t with sup_off[t] <= s
+  // track of this support: last t with sup_off[t] <= s (its own loop: through last_le the kernel's SASS changes)
   int64_t lo = 0, hi = p.T;
   while (hi - lo > 1) {
     const int64_t mid = (lo + hi) >> 1;
@@ -251,12 +251,7 @@ LM_D double fit_depth(const FitView &w, const double *p) { // CameraPose::projde
 __global__ void fit_prep_kernel(const __grid_constant__ FitPrepParams p) {
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= p.n) return;
-  int lo = 0, hi = p.V; // view of line g: last v with line_off[v] <= g
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (__ldg(&p.line_off[mid]) <= g) lo = mid; else hi = mid;
-  }
-  const FitView &w = p.views[lo];
+  const FitView &w = p.views[last_le<true>(p.line_off, p.V, g)]; // view of line g
   const double *l = p.lines3d + 6 * g;
   double *r = p.rec + 7 * g;
   for (int k = 0; k < 6; ++k) r[k] = l[k];

@@ -9,12 +9,7 @@ __global__ void sfm_pair_keys_kernel(const double *__restrict__ centres, const d
                                      const int64_t *__restrict__ rec_off, int64_t n_points, int64_t n_rec,
                                      unsigned long long *__restrict__ keys, unsigned int *__restrict__ num_points) {
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_rec; r += (int64_t)gridDim.x * blockDim.x) {
-    int64_t lo = 0, hi = n_points; // largest p with rec_off[p] <= r
-    while (hi - lo > 1) {
-      const int64_t mid = (lo + hi) >> 1;
-      if (rec_off[mid] <= r) lo = mid; else hi = mid;
-    }
-    const int64_t p = lo;
+    const int64_t p = last_le(rec_off, n_points, r);
     const int64_t k = r - rec_off[p]; // pair index in the track: (a, b), a > b, k = a (a - 1) / 2 + b
     int64_t a = (int64_t)((1.0 + sqrt(1.0 + 8.0 * (double)k)) * 0.5);
     while (a * (a - 1) / 2 > k) --a;

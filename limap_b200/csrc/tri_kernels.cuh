@@ -18,7 +18,6 @@ template <typename T> struct ViewT {
   T pad;
 };
 typedef ViewT<double> ViewD;
-typedef ViewT<float> ViewF;
 
 struct NodeRecord { // == lm_node_record
   double line[9];   // start3, end3, depths2, uncertainty
@@ -77,13 +76,17 @@ struct EdgeParams {
   LinkerDev<double> l3d; // linker3d_config after set_to_spatial_merging()
 };
 
+// Layout of the node kernel's candidate staging. tri_fast: the fast instantiation (reduced-form scorer, plane-pair
+// triangulation) runs. tri_cap_step: staging capacities are multiples of it. tri_smem_bytes: shared memory at capacity cap.
+bool tri_fast(const TriParams &p);
+int tri_cap_step(bool fast);
 size_t tri_smem_bytes(int cap, bool fast);
 void launch_group_edges(const uint8_t *row_state, const uint32_t *row_ng, const uint32_t *node_row_off,
                         const uint32_t *local_off, unsigned int *totals, int g, int64_t shard_node_begin, int64_t node_lo,
                         int64_t n, int ns, uint32_t *edge_off, uint32_t *edge_ng, cudaStream_t s);
 void launch_scene_prepare(const double *segs_raw, int64_t n_nodes, double add, const int64_t *line_off, int n_views,
                           double *segs, uint16_t *node_view, cudaStream_t s);
-cudaError_t launch_tri_node_kernel(const TriParams &p, int grid, int block, size_t smem, cudaStream_t s);
+cudaError_t launch_tri_node_kernel(const TriParams &p, int grid, size_t smem, cudaStream_t s);
 void launch_expand_rows(const int32_t *d_pairs, const int64_t *d_blk_row_off, const int32_t *d_blk_src_view,
                         const int32_t *d_blk_ng_view, const int64_t *d_blk_pair_off, int n_blocks,
                         const int64_t *d_line_off, int64_t r_begin, int64_t r_end, uint32_t *d_key, uint32_t *d_val,
@@ -94,9 +97,6 @@ void launch_expand_exhaustive(const int64_t *d_blk_row_off, const int32_t *d_blk
 void launch_node_offsets(const uint32_t *d_sorted_key, int64_t n_rows, int64_t row_base, int64_t node_lo,
                          int64_t node_hi, uint32_t *d_node_row_off, unsigned int *d_max_rows, cudaStream_t s);
 void launch_extract_nvalid(const NodeRecord *nodes, int64_t node_begin, int64_t n, uint32_t *out, cudaStream_t s);
-void launch_compact_edges_only(const uint8_t *row_state, const uint32_t *row_ng, const uint32_t *node_row_off,
-                               const uint32_t *edge_off, int64_t node_begin, int64_t n, int ns, uint32_t *edge_ng,
-                               cudaStream_t s);
 void launch_edge_pairs(const uint32_t *edge_off, const uint32_t *edge_ng, const int64_t *line_off,
                        int64_t node_begin, int64_t n_nodes, int64_t n_edges, int64_t *out, cudaStream_t s);
 void launch_edges_for_host(const uint32_t *edge_off, const uint32_t *edge_ng, const int32_t *img_ids,
