@@ -25,6 +25,7 @@ import pytest
 from limap_b200.config import DEFAULT_YAML_TRIANGULATION
 from limap_b200.synth import make_scene
 
+import boundary_scenes
 from parity_utils import compare_nodes, compare_tracks
 
 from oracle import oracle as orc
@@ -233,6 +234,28 @@ def test_boundary_3d_oracle_equals_compiled_reference(name):
     r = _StoredTri(_gold("boundary_3d_" + name), sc, every=1)
     check_planted(r, sc, planted)
     compare_stored(sc, r, o, 1e-7)
+
+
+def _ref_planted(name):
+    from boundary_scenes import planted_cfg, planted_scene
+    sc, _ = planted_scene(name)
+    return _record_tri(_feed(ref.RefTri(planted_cfg(name), threads=1), sc), sc, every=1)
+
+
+@pytest.mark.parametrize("name", sorted(boundary_scenes.PLANTED))
+def test_boundary_planted_oracle_equals_compiled_reference(name):
+    """Phase-A gates (ray-plane angle at 1 and 5 deg, epipolar IoU, also with grazing epipolar lines, sensitivity),
+    2D linker sub-tests (angle below and above the 14.4775 deg switch, overlap, smart angle, perpendicular distance) and
+    fullscore_th planted at their thresholds (tests/boundary_scenes.py), at depths ~1 and ~1e3 and at asset-unit
+    coordinates: the reference's compiled code decides every planted row as intended, and the oracle reproduces its
+    candidate lists, valid connections and tracks bit-exact, endpoints within 1e-7, scores within 1e-9 (1e-8 where the
+    epipolar lines graze)."""
+    from boundary_scenes import check_planted_family, checked_planted_scene, planted_cfg, planted_golden, planted_score_tol
+    sc, planted = checked_planted_scene(name)
+    r = _StoredTri(_gold(planted_golden(name)), sc, every=1)
+    check_planted_family(name, r, sc, planted)
+    o = _feed(orc.OracleTri(planted_cfg(name), threads=1), sc)
+    compare_stored(sc, r, o, 1e-7, planted_score_tol(name))
 
 
 def test_boundary_min_length_oracle_equals_compiled_reference():
@@ -1043,6 +1066,8 @@ REFERENCE_OUTPUTS = {**{"pipeline_" + name: (lambda name=name: _ref_pipeline(nam
                      "boundary_min_length": _ref_boundary_min_length,
                      **{"boundary_3d_" + name: (lambda name=name: _ref_boundary_3d(name))
                         for name in ("angle_10", "angle_14.4775", "angle_20", "scaleinv")},
+                     **{boundary_scenes.planted_golden(name): (lambda name=name: _ref_planted(name))
+                        for name in sorted(boundary_scenes.PLANTED)},
                      "two_view": _ref_two_view, "camera": _ref_camera, "linker": _ref_linker, "aggregate": _ref_aggregate,
                      "residuals": _ref_residuals, "filters": _ref_filters, "sfm": _ref_sfm, "vp": _ref_vp,
                      "linetrack": _ref_linetrack, "value_types": _ref_value_types, "track_filters": _ref_track_filters,
