@@ -50,11 +50,6 @@ void make_view(int model_id, const double *kv, const double *qv, const double *t
   d.pad = 0;
 }
 
-static int sync_stream(lm_ctx *c) {
-  CU(cudaStreamSynchronize(c->stream));
-  return LM_OK;
-}
-
 int fetch_nodes(lm_ctx *c) {
   if (c->h_nodes_valid) return LM_OK;
   c->h_nodes.resize(c->n_nodes);
@@ -204,7 +199,8 @@ int lm_ctx_synchronize(lm_ctx *c) {
   if (!c) return fail(LM_ERR_INVALID, "ctx is NULL");
   CU(cudaSetDevice(c->device));
   CU(cudaStreamSynchronize(c->copy_stream));
-  return sync_stream(c);
+  CU(cudaStreamSynchronize(c->stream));
+  return LM_OK;
 }
 
 static int tri_clear_impl(lm_ctx *c, bool sync_copies);
@@ -262,7 +258,6 @@ int lm_scene_upload(lm_ctx *c, int32_t n_views, const int32_t *img_ids, const in
   int rc = upload_segs(c, true);
   if (rc) return rc;
   c->image_added.assign(n_views, 0);
-  c->image_norder.assign(n_views, 0);
   c->stats.n_nodes = c->n_nodes;
   return tri_clear_impl(c, false); // (both streams were drained on entry: no match chunk is in flight)
 }
@@ -341,7 +336,6 @@ static int tri_clear_impl(lm_ctx *c, bool sync_copies) {
   c->blocks.clear();
   c->raw_uploaded = 0;
   std::fill(c->image_added.begin(), c->image_added.end(), 0);
-  std::fill(c->image_norder.begin(), c->image_norder.end(), 0);
   if (c->copy_stream && sync_copies) cudaStreamSynchronize(c->copy_stream); // (the chunk events go back to the pool)
   for (auto &ch : c->chunks) c->event_pool.push_back(ch.ev);
   c->chunks.clear();
@@ -384,15 +378,9 @@ static int upload_raw_blocks(lm_ctx *c) {
     CU(c->d_raw_blocks.grow_keep(std::max<size_t>((size_t)n * sizeof(lm::RawBlock) * 2, 1 << 16),
                                  c->raw_uploaded * sizeof(lm::RawBlock), c->stream));
   }
-  std::vector<lm::RawBlock> tmp(n - c->raw_uploaded);
-  for (int64_t i = c->raw_uploaded; i < n; ++i) {
-    const MatchBlock &b = c->blocks[i];
-    lm::RawBlock &r = tmp[i - c->raw_uploaded];
-    r.src_view = b.src_view; r.ng_view = b.ng_view; r.n_rows = b.n_rows; r.pair_off = b.pair_off; r.order = b.order; r.pad = 0;
-  }
-  // pageable source: the runtime stages it, so `tmp` may die at scope exit
-  CU(cudaMemcpyAsync(c->d_raw_blocks.as<lm::RawBlock>() + c->raw_uploaded, tmp.data(), tmp.size() * sizeof(lm::RawBlock),
-                     cudaMemcpyHostToDevice, c->copy_stream));
+  // pageable source: the runtime stages it before returning, so `blocks` may grow (and move) afterwards
+  CU(cudaMemcpyAsync(c->d_raw_blocks.as<lm::RawBlock>() + c->raw_uploaded, c->blocks.data() + c->raw_uploaded,
+                     (n - c->raw_uploaded) * sizeof(lm::RawBlock), cudaMemcpyHostToDevice, c->copy_stream));
   if (!c->ev_raw) CU(cudaEventCreateWithFlags(&c->ev_raw, cudaEventDisableTiming));
   CU(cudaEventRecord(c->ev_raw, c->copy_stream));
   c->raw_uploaded = n;
@@ -408,20 +396,34 @@ static int upload_pairs(lm_ctx *c, const int32_t *pairs, int64_t total, bool on_
   }
   // one event per copy; the copies start at 2 MB and double up to 16 MB, so that the first pipeline group of a run (a few
   // per cent of the rows) does not wait for a full-size chunk
-  const int64_t kChunk = 2 << 20, kEventEvery = 1;
-  int64_t k = 0, step = 256 << 10;
-  for (int64_t o = 0, n = 0; o < total; o += n, ++k, step = std::min(kChunk, step * 2)) {
+  const int64_t kChunk = 2 << 20;
+  int64_t step = 256 << 10;
+  for (int64_t o = 0, n = 0; o < total; o += n, step = std::min(kChunk, step * 2)) {
     n = std::min(step, total - o);
     CU(cudaMemcpyAsync(c->d_pairs.as<char>() + (c->pairs_rows + o) * 8, pairs + 2 * o, n * 8,
                        on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->copy_stream));
-    if ((k + 1) % kEventEvery == 0 || o + n >= total) {
-      cudaEvent_t ev;
-      if (!c->event_pool.empty()) { ev = c->event_pool.back(); c->event_pool.pop_back(); }
-      else CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-      CU(cudaEventRecord(ev, c->copy_stream));
-      c->chunks.push_back({c->pairs_rows + o + n, ev});
-    }
+    cudaEvent_t ev;
+    if (!c->event_pool.empty()) { ev = c->event_pool.back(); c->event_pool.pop_back(); }
+    else CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    CU(cudaEventRecord(ev, c->copy_stream));
+    c->chunks.push_back({c->pairs_rows + o + n, ev});
   }
+  return LM_OK;
+}
+
+// The shared tail of the match-based entry points, once their arguments are validated: append the blocks (pair_off
+// already counts from the start of the device store), upload their descriptors and then `total` rows of `pairs`, and
+// mark the blocks' source images as triangulated.
+static int append_matches(lm_ctx *c, const std::vector<lm::RawBlock> &nb, const int32_t *pairs, int64_t total,
+                          bool on_device) {
+  c->blocks.insert(c->blocks.end(), nb.begin(), nb.end());
+  int rc = upload_raw_blocks(c);
+  if (!rc) rc = upload_pairs(c, pairs, total, on_device);
+  if (rc) return rc;
+  c->pairs_rows += total;
+  for (const lm::RawBlock &b : nb) c->image_added[b.src_view] = 1;
+  c->any_matches = true;
+  c->ran = false;
   return LM_OK;
 }
 
@@ -437,31 +439,18 @@ static int add_matches_impl(lm_ctx *c, int32_t img_id, int32_t n_ng, const int32
   if (c->any_exhaustive) return fail(LM_ERR_STATE, "cannot mix exhaustive and match-based triangulation in one run");
   const int64_t total = n_ng > 0 ? row_off[n_ng] : 0;
   std::set<int> seen;
+  std::vector<lm::RawBlock> nb;
   for (int g = 0; g < n_ng; ++g) {
-    if (c->id2view.find(ng_ids[g]) == c->id2view.end())
-      return fail(LM_ERR_INVALID, "unknown neighbor image id " + std::to_string(ng_ids[g]));
+    auto f = c->id2view.find(ng_ids[g]);
+    if (f == c->id2view.end()) return fail(LM_ERR_INVALID, "unknown neighbor image id " + std::to_string(ng_ids[g]));
     if (!seen.insert(ng_ids[g]).second) return fail(LM_ERR_INVALID, "duplicate neighbor id in one TriangulateImage call");
     if (row_off[g + 1] < row_off[g]) return fail(LM_ERR_INVALID, "row_off must be non-decreasing");
+    // order 0: the run visits neighbours in ascending id = std::map order (base_line_triangulator.cc:74)
+    nb.push_back({sv, f->second, row_off[g + 1] - row_off[g], c->pairs_rows + row_off[g], 0, 0});
   }
-  for (int g = 0; g < n_ng; ++g) {
-    MatchBlock b;
-    b.src_view = sv;
-    b.ng_view = c->id2view[ng_ids[g]];
-    b.n_rows = row_off[g + 1] - row_off[g];
-    b.pair_off = c->pairs_rows + row_off[g];
-    b.order = 0; // std::map order = ascending neighbour id (base_line_triangulator.cc:74)
-    c->blocks.push_back(b);
-  }
-  {
-    int rc_ = upload_raw_blocks(c);
-    if (!rc_) rc_ = upload_pairs(c, pairs, total, on_device);
-    if (rc_) return rc_;
-  }
-  c->pairs_rows += total;
-  c->image_added[sv] = 1;
-  c->any_matches = true;
-  c->ran = false;
-  return LM_OK;
+  const int rc = append_matches(c, nb, pairs, total, on_device);
+  if (!rc) c->image_added[sv] = 1; // (an image without neighbours, too)
+  return rc;
 }
 int lm_tri_add_image_matches(lm_ctx *c, int32_t img_id, int32_t n_ng, const int32_t *ng_ids, const int64_t *row_off,
                              const int32_t *pairs) {
@@ -478,31 +467,16 @@ int lm_tri_add_matches_bulk(lm_ctx *c, int32_t n_blocks, const int32_t *src_img_
   if (c->any_exhaustive) return fail(LM_ERR_STATE, "cannot mix exhaustive and match-based triangulation in one run");
   CU(cudaSetDevice(c->device));
   const int64_t total = n_blocks > 0 ? row_off[n_blocks] : 0;
-  std::vector<char> seen_img(c->V, 0);
-  std::vector<MatchBlock> nb;
+  std::vector<lm::RawBlock> nb;
   nb.reserve(n_blocks);
   for (int b = 0; b < n_blocks; ++b) {
     auto is = c->id2view.find(src_img_ids[b]), in_ = c->id2view.find(ng_img_ids[b]);
     if (is == c->id2view.end() || in_ == c->id2view.end()) return fail(LM_ERR_INVALID, "unknown image id in matches");
     if (c->image_added[is->second]) return fail(LM_ERR_STATE, "image " + std::to_string(src_img_ids[b]) + " was already triangulated");
     if (row_off[b + 1] < row_off[b]) return fail(LM_ERR_INVALID, "row_off must be non-decreasing");
-    seen_img[is->second] = 1;
-    MatchBlock m;
-    m.src_view = is->second; m.ng_view = in_->second; m.n_rows = row_off[b + 1] - row_off[b];
-    m.pair_off = c->pairs_rows + row_off[b]; m.order = 0;
-    nb.push_back(m);
+    nb.push_back({is->second, in_->second, row_off[b + 1] - row_off[b], c->pairs_rows + row_off[b], 0, 0});
   }
-  c->blocks.insert(c->blocks.end(), nb.begin(), nb.end());
-  {
-    int rc_ = upload_raw_blocks(c);
-    if (!rc_) rc_ = upload_pairs(c, pairs, total, false);
-    if (rc_) return rc_;
-  }
-  c->pairs_rows += total;
-  for (int v = 0; v < c->V; ++v) if (seen_img[v]) c->image_added[v] = 1;
-  c->any_matches = true;
-  c->ran = false;
-  return LM_OK;
+  return append_matches(c, nb, pairs, total, false);
 }
 
 int lm_tri_get_nodes(lm_ctx *c, lm_node_record *out) {
@@ -548,364 +522,345 @@ int lm_tri_add_image_exhaustive(lm_ctx *c, int32_t img_id, int32_t n_ng, const i
   if (c->image_added[sv]) return fail(LM_ERR_STATE, "image " + std::to_string(img_id) + " was already triangulated");
   if (c->any_matches) return fail(LM_ERR_STATE, "cannot mix exhaustive and match-based triangulation in one run");
   const int64_t nl = c->line_off[sv + 1] - c->line_off[sv];
+  std::vector<lm::RawBlock> nb;
   for (int g = 0; g < n_ng; ++g) {
     auto f = c->id2view.find(ng_ids[g]);
     if (f == c->id2view.end()) return fail(LM_ERR_INVALID, "unknown neighbor image id " + std::to_string(ng_ids[g]));
-    MatchBlock b;
-    b.src_view = sv;
-    b.ng_view = f->second;
-    b.n_rows = nl * (c->line_off[b.ng_view + 1] - c->line_off[b.ng_view]);
-    b.pair_off = -1;
-    b.order = g; // neighbours are visited in the given order (base_line_triangulator.cc:116-117)
-    c->blocks.push_back(b);
+    // no stored pairs; order g: neighbours are visited in the given order (base_line_triangulator.cc:116-117)
+    nb.push_back({sv, f->second, nl * (c->line_off[f->second + 1] - c->line_off[f->second]), -1, g, 0});
   }
+  c->blocks.insert(c->blocks.end(), nb.begin(), nb.end());
   c->image_added[sv] = 1;
   c->any_exhaustive = true;
   c->ran = false;
   return upload_raw_blocks(c);
 }
 
-int lm_tri_run(lm_ctx *c) {
-  if (!c) return fail(LM_ERR_INVALID, "ctx is NULL");
-  if (!c->have_scene) return fail(LM_ERR_STATE, "no scene uploaded");
-  if (!c->have_cfg) return fail(LM_ERR_STATE, "lm_tri_configure must precede lm_tri_run");
-  CU(cudaSetDevice(c->device));
-  cudaStream_t s = c->stream;
-  const int vb = std::max(0, c->shard_begin), ve = (c->shard_end < 0) ? c->V : std::min(c->V, c->shard_end);
-  // blocks of this shard in flat order: (source view, neighbour order)
-  std::vector<MatchBlock> blk;
-  for (const MatchBlock &b : c->blocks)
-    if (b.src_view >= vb && b.src_view < ve) blk.push_back(b);
-  const bool exhaustive = c->any_exhaustive;
-  std::stable_sort(blk.begin(), blk.end(), [exhaustive](const MatchBlock &a, const MatchBlock &b) {
+// ---- lm_tri_run, one function per stage ---------------------------------------------------------------------------
+// What a run covers: the blocks of the shard's source views [vb, ve) in flat order (source view, neighbour order).
+struct RunPlan {
+  int vb = 0, ve = 0, ns = 1;    // ns: proposal slots per match row (3 with VP proposals)
+  bool exhaustive = false;
+  std::vector<lm::RawBlock> blk; // the blocks in flat order
+  std::vector<int64_t> row_off;  // first flat row of every block; row_off[nb] = n_rows
+  int nb = 0, n_groups = 1;      // blocks, pipeline groups
+  int64_t n_rows = 0;
+  int node_bits = 1;             // key bits of the row sort by node id
+};
+
+// What one attempt of the run queued (a staging overflow repeats the run once): whether tri_node_kernel's fast
+// instantiation runs, its staging capacity (candidate slots per node), the launches, the groups that ran the kernel.
+struct Attempt {
+  bool fast = false;
+  int cap = 0, launches = 0;
+  std::vector<char> group_has_kernel;
+};
+
+static int plan_run(const lm_ctx &c, RunPlan &r) {
+  r.vb = std::max(0, c.shard_begin);
+  r.ve = (c.shard_end < 0) ? c.V : std::min(c.V, c.shard_end);
+  r.exhaustive = c.any_exhaustive;
+  r.ns = (c.cfg.use_vp && !c.cfg.disable_vp_triangulation && c.have_vps) ? 3 : 1;
+  for (const lm::RawBlock &b : c.blocks)
+    if (b.src_view >= r.vb && b.src_view < r.ve) r.blk.push_back(b);
+  std::stable_sort(r.blk.begin(), r.blk.end(), [&r](const lm::RawBlock &a, const lm::RawBlock &b) {
     if (a.src_view != b.src_view) return a.src_view < b.src_view;
-    if (exhaustive) return a.order < b.order;
+    if (r.exhaustive) return a.order < b.order;
     return a.ng_view < b.ng_view;
   });
-  const int nb = (int)blk.size();
-  std::vector<int64_t> row_off(nb + 1, 0), pair_off(nb);
-  std::vector<int32_t> bsrc(nb), bng(nb);
-  for (int i = 0; i < nb; ++i) {
-    row_off[i + 1] = row_off[i] + blk[i].n_rows;
-    pair_off[i] = blk[i].pair_off;
-    bsrc[i] = blk[i].src_view;
-    bng[i] = blk[i].ng_view;
-  }
-  const int64_t n_rows = row_off[nb];
+  r.nb = (int)r.blk.size();
+  r.row_off.assign(r.nb + 1, 0);
+  for (int i = 0; i < r.nb; ++i) r.row_off[i + 1] = r.row_off[i] + r.blk[i].n_rows;
+  r.n_rows = r.row_off[r.nb];
   // the sort and scan item counts are 32-bit signed
-  if (n_rows >= ((int64_t)1 << 31) - 64) return fail(LM_ERR_INVALID, "more than 2^31 match rows in one run (shard the scene by source image)");
-  c->n_rows = n_rows;
-  c->node_begin = c->line_off[vb];
-  c->node_end = c->line_off[ve];
-  c->h_nodes_valid = c->h_rows_valid = c->h_edges_valid = false;
-  c->edges_collected = false;
-  c->edges_count_on_device = false;
-  c->tracks.clear();
+  if (r.n_rows >= ((int64_t)1 << 31) - 64) return fail(LM_ERR_INVALID, "more than 2^31 match rows in one run (shard the scene by source image)");
+  r.n_groups = r.exhaustive ? 1 : (int)std::max<int64_t>(1, std::min<int64_t>(c.pipeline_groups, r.n_rows >> 16));
+  while (((int64_t)1 << r.node_bits) < c.n_nodes) ++r.node_bits;
+  return LM_OK;
+}
 
+// Every device buffer and event of the run but the slab, whose size depends on the staging capacity.
+static int ensure_run_buffers(lm_ctx *c, const RunPlan &r) {
+  const int nb = r.nb, n_all = (int)c->blocks.size();
+  const int64_t rows = std::max<int64_t>(r.n_rows, 1), slots = std::max<int64_t>(r.n_rows * r.ns, 1);
+  const int64_t n_shard_nodes = c->node_end - c->node_begin;
   CU(c->d_blk_row_off.ensure(8 * (nb + 1)));
   CU(c->d_blk_src.ensure(4 * std::max(nb + 1, 2)));
   CU(c->d_blk_ng.ensure(4 * std::max(nb + 1, 2)));
   CU(c->d_blk_pair_off.ensure(8 * std::max(nb, 1)));
-  CU(c->d_key.ensure(4 * std::max<int64_t>(n_rows, 1)));
-  CU(c->d_key2.ensure(4 * std::max<int64_t>(n_rows, 1)));
-  CU(c->d_val.ensure(4 * std::max<int64_t>(n_rows, 1)));
-  CU(c->d_val2.ensure(4 * std::max<int64_t>(n_rows, 1)));
+  CU(c->d_key.ensure(4 * rows)); CU(c->d_key2.ensure(4 * rows));
+  CU(c->d_val.ensure(4 * rows)); CU(c->d_val2.ensure(4 * rows));
   CU(c->d_node_row_off.ensure(4 * (c->n_nodes + 2)));
   CU(c->d_scalars.ensure(1024));
   CU(c->d_nodes.ensure(sizeof(lm::NodeRecord) * std::max<int64_t>(c->n_nodes, 1)));
-  const int ns = (c->cfg.use_vp && !c->cfg.disable_vp_triangulation && c->have_vps) ? 3 : 1;
-  c->ns = ns;
-  CU(c->d_row_state.ensure(std::max<int64_t>(n_rows * ns, 1)));
-  if (c->cfg.debug_mode) CU(c->d_row_cand.ensure(80 * std::max<int64_t>(n_rows * ns, 1)));
-
-  CU(cudaEventRecord(c->ev0, s));
-  // Two compute streams: `sp` prepares the rows of a pipeline group (expansion, sort, node offsets), `s` runs the node
-  // kernels. The preparation of group g+1 is queued right behind that of group g, so it executes under the node kernel of
-  // group g; everything `sp` touches is per-group slices, its own scratch, or is read by `s` only after the group's event.
-  cudaStream_t sp = c->prep_stream;
-  CU(cudaEventRecord(c->ev_run_begin, s)); // whatever the caller queued on the engine's stream comes first
-  CU(cudaStreamWaitEvent(sp, c->ev_run_begin, 0));
-  // scene tables / VP tables travel on the copy stream (see lm_ctx::ev_scene)
-  CU(cudaStreamWaitEvent(sp, c->ev_scene, 0));
-  CU(cudaStreamWaitEvent(s, c->ev_scene, 0));
-  lm::launch_zero_words(c->d_scalars.p, 256, sp);
-  // block tables, derived on the device from the descriptors uploaded with the matches (no transfer now)
-  {
-    const int n_all = (int)c->blocks.size();
-    CU(c->d_blk_rows.ensure(8 * (nb + 2)));
-    if (n_all) {
-      CU(c->d_bkey.ensure(4 * n_all)); CU(c->d_bkey2.ensure(4 * n_all));
-      CU(c->d_bval.ensure(4 * n_all)); CU(c->d_bval2.ensure(4 * n_all));
-      // the descriptors travel on the copy stream ahead of their matches (bulk add: ahead of all matches)
-      if (c->ev_raw) CU(cudaStreamWaitEvent(sp, c->ev_raw, 0));
-      lm::launch_block_keys(c->d_raw_blocks.as<lm::RawBlock>(), n_all, vb, ve, exhaustive ? 1 : 0, c->d_bkey.as<uint32_t>(),
-                            c->d_bval.as<uint32_t>(), sp);
-      cub::DoubleBuffer<uint32_t> bk(c->d_bkey.as<uint32_t>(), c->d_bkey2.as<uint32_t>());
-      cub::DoubleBuffer<uint32_t> bv(c->d_bval.as<uint32_t>(), c->d_bval2.as<uint32_t>());
-      CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, bk, bv, n_all, 0, 32, sp); }));
-      lm::launch_block_gather(c->d_raw_blocks.as<lm::RawBlock>(), bv.Current(), nb, c->d_blk_src.as<int32_t>(),
-                              c->d_blk_ng.as<int32_t>(), c->d_blk_pair_off.as<int64_t>(), c->d_blk_rows.as<int64_t>(), sp);
-    } else {
-      lm::launch_zero_words(c->d_blk_rows.p, 4, sp);
-    }
-    CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) {
-      return cub::DeviceScan::ExclusiveSum(t, b, c->d_blk_rows.as<int64_t>(), c->d_blk_row_off.as<int64_t>(), nb + 1, sp);
-    }));
+  CU(c->d_row_state.ensure(slots));
+  if (c->cfg.debug_mode) CU(c->d_row_cand.ensure(80 * slots));
+  CU(c->d_blk_rows.ensure(8 * (nb + 2)));
+  if (n_all) {
+    CU(c->d_bkey.ensure(4 * n_all)); CU(c->d_bkey2.ensure(4 * n_all));
+    CU(c->d_bval.ensure(4 * n_all)); CU(c->d_bval2.ensure(4 * n_all));
   }
-  // d_scalars words: [1] index error, [2] staging overflow, bytes 16..47 counters, words [16 + g] largest node of group g
-  int *d_err = c->d_scalars.as<int>() + 1;
-  unsigned long long *d_counters = reinterpret_cast<unsigned long long *>(c->d_scalars.as<char>() + 16);
-  int launches = 0;
+  for (cudaEvent_t e; (int)c->evk.size() < 2 * r.n_groups; c->evk.push_back(e)) CU(cudaEventCreate(&e));
+  for (cudaEvent_t e; (int)c->evp.size() < r.n_groups; c->evp.push_back(e))
+    CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  const size_t shard_bytes = 4 * (n_shard_nodes + 2);
+  CU(c->d_nvalid.ensure(shard_bytes)); CU(c->d_local_off.ensure(shard_bytes)); CU(c->d_edge_off.ensure(shard_bytes));
+  CU(c->d_edge_ng.ensure(4 * slots));
+  return LM_OK;
+}
+
+// The shard's block tables, derived on the prepare stream from the descriptors uploaded with the matches (no transfer
+// now): keys by (source view, neighbour order), CUB sort, gather, and the exclusive scan of the rows.
+static int queue_block_tables(lm_ctx *c, const RunPlan &r) {
+  cudaStream_t sp = c->prep_stream;
+  const int nb = r.nb, n_all = (int)c->blocks.size();
+  if (n_all) {
+    // the descriptors travel on the copy stream ahead of their matches (bulk add: ahead of all matches)
+    if (c->ev_raw) CU(cudaStreamWaitEvent(sp, c->ev_raw, 0));
+    lm::launch_block_keys(c->d_raw_blocks.as<lm::RawBlock>(), n_all, r.vb, r.ve, r.exhaustive ? 1 : 0,
+                          c->d_bkey.as<uint32_t>(), c->d_bval.as<uint32_t>(), sp);
+    cub::DoubleBuffer<uint32_t> bk(c->d_bkey.as<uint32_t>(), c->d_bkey2.as<uint32_t>());
+    cub::DoubleBuffer<uint32_t> bv(c->d_bval.as<uint32_t>(), c->d_bval2.as<uint32_t>());
+    CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, bk, bv, n_all, 0, 32, sp); }));
+    lm::launch_block_gather(c->d_raw_blocks.as<lm::RawBlock>(), bv.Current(), nb, c->d_blk_src.as<int32_t>(),
+                            c->d_blk_ng.as<int32_t>(), c->d_blk_pair_off.as<int64_t>(), c->d_blk_rows.as<int64_t>(), sp);
+  } else {
+    lm::launch_zero_words(c->d_blk_rows.p, 4, sp);
+  }
+  CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, c->d_blk_rows.as<int64_t>(), c->d_blk_row_off.as<int64_t>(), nb + 1, sp);
+  }));
+  return LM_OK;
+}
+
+// The node kernel's parameters that come from the context and the configuration, including the constants derived from
+// the configuration. queue_group sets the per-group ones (node range, staging capacity, slab).
+static lm::TriParams make_tri_params(const lm_ctx &c, int ns) {
   lm::TriParams p;
   memset(&p, 0, sizeof(p));
-  p.views = c->d_views.as<lm::ViewD>();
-  p.segs = c->d_segs.as<double4>();
-  p.node_view = c->d_node_view.as<uint16_t>();
-  p.line_off = c->d_line_off.as<int64_t>();
-  p.node_row_off = c->d_node_row_off.as<uint32_t>();
-  p.nodes = c->d_nodes.as<lm::NodeRecord>();
-  p.row_state = c->d_row_state.as<uint8_t>();
-  p.row_cand = c->cfg.debug_mode ? c->d_row_cand.as<double>() : nullptr;
-  p.counters = d_counters;
-  p.overflow = c->d_scalars.as<int>() + 2;
-  p.node_begin = c->node_begin;
-  p.node_end = c->node_end;
-  const lm_tri_config &g = c->cfg;
+  p.views = c.d_views.as<lm::ViewD>();
+  p.segs = c.d_segs.as<double4>();
+  p.node_view = c.d_node_view.as<uint16_t>();
+  p.line_off = c.d_line_off.as<int64_t>();
+  p.node_row_off = c.d_node_row_off.as<uint32_t>();
+  p.nodes = c.d_nodes.as<lm::NodeRecord>();
+  p.row_state = c.d_row_state.as<uint8_t>();
+  p.row_cand = c.cfg.debug_mode ? c.d_row_cand.as<double>() : nullptr;
+  p.row_ng = c.sorted_val;
+  // d_scalars words: [1] index error, [2] staging overflow, bytes 16..47 counters, words [16 + g] largest node of group g
+  p.counters = reinterpret_cast<unsigned long long *>(c.d_scalars.as<char>() + 16);
+  p.overflow = c.d_scalars.as<int>() + 2;
+  p.node_begin = c.node_begin;
+  p.node_end = c.node_end;
+  const lm_tri_config &g = c.cfg;
   p.min_length_2d = g.min_length_2d; p.line_tri_angle_threshold = g.line_tri_angle_threshold;
   p.IoU_threshold = g.IoU_threshold; p.sensitivity_threshold = g.sensitivity_threshold; p.var2d = g.var2d;
   p.fullscore_th = g.fullscore_th; p.max_valid_conns = g.max_valid_conns;
   p.use_endpoints_triangulation = g.use_endpoints_triangulation; p.disable_algebraic = g.disable_algebraic_triangulation;
   p.use_vp = (ns == 3); p.disable_vp = g.disable_vp_triangulation;
-  p.vp_label = c->d_vp_label.as<int32_t>(); p.vp_off = c->d_vp_voff.as<int64_t>(); p.vps = c->d_vp_vps.as<double>();
-  p.ranges_flag = c->ranges_flag;
-  for (int i = 0; i < 3; ++i) { p.rlo[i] = c->rlo[i]; p.rhi[i] = c->rhi[i]; }
+  p.vp_label = c.d_vp_label.as<int32_t>(); p.vp_off = c.d_vp_voff.as<int64_t>(); p.vps = c.d_vp_vps.as<double>();
+  p.ranges_flag = c.ranges_flag;
+  for (int i = 0; i < 3; ++i) { p.rlo[i] = c.rlo[i]; p.rhi[i] = c.rhi[i]; }
   p.l2d = to_dev<double>(g.linker2d);
-  {
-    lm_linker_config l3 = g.linker3d; // set_to_shared_parent_scoring (line_linker.h:115-121)
-    l3.use_angle = 1; l3.use_overlap = 0; l3.use_perp = 0; l3.use_innerseg = 0; l3.use_scaleinv = 1;
-    p.l3d = to_dev<double>(l3);
+  lm_linker_config l3 = g.linker3d; // set_to_shared_parent_scoring (line_linker.h:115-121)
+  l3.use_angle = 1; l3.use_overlap = 0; l3.use_perp = 0; l3.use_innerseg = 0; l3.use_scaleinv = 1;
+  p.l3d = to_dev<double>(l3);
+  const double kPi = 3.14159265358979323846;
+  const double t3 = p.l3d.th_angle, t2 = p.l2d.th_angle;
+  p.cos_th3d_f = (t3 >= 90.0) ? -1.0f : (float)(std::cos(t3 * kPi / 180.0) - 4e-6);
+  const double c2 = (t2 >= 90.0) ? 0.0 : std::cos(t2 * kPi / 180.0);
+  p.cos2_th2d = c2 * c2;
+  p.th_perp2_2d = p.l2d.th_perp * p.l2d.th_perp;
+  const double ta = p.line_tri_angle_threshold, tsn = p.sensitivity_threshold;
+  p.tri_poly_ok = (ta > 0.0 && ta < 90.0);
+  p.sens_poly_ok = (tsn > 0.0 && tsn < 90.0);
+  p.sin2_tri = std::sin(ta * kPi / 180.0) * std::sin(ta * kPi / 180.0);
+  p.sin2_sens = std::sin(tsn * kPi / 180.0) * std::sin(tsn * kPi / 180.0);
+  p.fast_forms = (p.l2d.use_innerseg || getenv("LIMAP_B200_REFERENCE_FORMS")) ? 0 : 1;
+  p.inv_sig_a3 = 1.0 / (p.l3d.th_angle * p.l3d.mult);
+  p.inv_sig_s3 = 1.0 / (p.l3d.th_scaleinv * p.l3d.mult);
+  p.inv_sig_a2 = 1.0 / (p.l2d.th_angle * p.l2d.mult);
+  p.inv_sig_p2 = 1.0 / (p.l2d.th_perp * p.l2d.mult);
+  p.q_cut3 = -2.0 * std::log(p.l3d.score_th) * (1.0 + 1e-9);
+  p.q_cut3_lo = -2.0 * std::log(p.l3d.score_th) * (1.0 - 1e-9);
+  p.q_cut2 = -2.0 * std::log(p.l2d.score_th) * (1.0 + 1e-9);
+  p.q_cut2_lo = -2.0 * std::log(p.l2d.score_th) * (1.0 - 1e-9);
+  p.inv_smart_den2 = 1.0 / (p.l2d.th_smartoverlap - p.l2d.th_overlap);
+  return p;
+}
+
+// Results outside the shard (filled by lm_tri_import_nodes in a multi-GPU run) start from the empty record, so a
+// getter never sees uninitialised memory; done once per scene/shard, imports survive later runs.
+static int clear_outside_shard(lm_ctx *c) {
+  if (c->outside_shard_clean || (c->node_begin <= 0 && c->node_end >= c->n_nodes)) return LM_OK;
+  cudaStream_t s = c->stream;
+  if (c->node_begin > 0) {
+    CU(cudaMemsetAsync(c->d_nodes.p, 0, sizeof(lm::NodeRecord) * c->node_begin, s));
+    CU(cudaMemsetAsync(c->d_node_row_off.p, 0, 4 * c->node_begin, s));
   }
-  {
-    const double kPi = 3.14159265358979323846;
-    const double t3 = p.l3d.th_angle, t2 = p.l2d.th_angle;
-    p.cos_th3d_f = (t3 >= 90.0) ? -1.0f : (float)(std::cos(t3 * kPi / 180.0) - 4e-6);
-    const double c2 = (t2 >= 90.0) ? 0.0 : std::cos(t2 * kPi / 180.0);
-    p.cos2_th2d = c2 * c2;
-    p.th_perp2_2d = p.l2d.th_perp * p.l2d.th_perp;
-    const double ta = p.line_tri_angle_threshold, tsn = p.sensitivity_threshold;
-    p.tri_poly_ok = (ta > 0.0 && ta < 90.0);
-    p.sens_poly_ok = (tsn > 0.0 && tsn < 90.0);
-    p.sin2_tri = std::sin(ta * kPi / 180.0) * std::sin(ta * kPi / 180.0);
-    p.sin2_sens = std::sin(tsn * kPi / 180.0) * std::sin(tsn * kPi / 180.0);
-    p.fast_forms = (p.l2d.use_innerseg || getenv("LIMAP_B200_REFERENCE_FORMS")) ? 0 : 1;
-    p.inv_sig_a3 = 1.0 / (p.l3d.th_angle * p.l3d.mult);
-    p.inv_sig_s3 = 1.0 / (p.l3d.th_scaleinv * p.l3d.mult);
-    p.inv_sig_a2 = 1.0 / (p.l2d.th_angle * p.l2d.mult);
-    p.inv_sig_p2 = 1.0 / (p.l2d.th_perp * p.l2d.mult);
-    p.q_cut3 = -2.0 * std::log(p.l3d.score_th) * (1.0 + 1e-9);
-    p.q_cut3_lo = -2.0 * std::log(p.l3d.score_th) * (1.0 - 1e-9);
-    p.q_cut2 = -2.0 * std::log(p.l2d.score_th) * (1.0 + 1e-9);
-    p.q_cut2_lo = -2.0 * std::log(p.l2d.score_th) * (1.0 - 1e-9);
-    p.inv_smart_den2 = 1.0 / (p.l2d.th_smartoverlap - p.l2d.th_overlap);
+  if (c->node_end < c->n_nodes) {
+    CU(cudaMemsetAsync(c->d_nodes.as<lm::NodeRecord>() + c->node_end, 0, sizeof(lm::NodeRecord) * (c->n_nodes - c->node_end), s));
+    CU(cudaMemsetAsync(c->d_node_row_off.as<uint32_t>() + c->node_end + 1, 0, 4 * (c->n_nodes - c->node_end), s));
   }
-  // ---- groups of source images: sort + node kernel of group g overlap the upload of group g+1 -----------
-  int nbits = 1;
-  while (((int64_t)1 << nbits) < c->n_nodes) ++nbits;
-  // canonical sorted buffers: d_key2 / d_val2
-  c->sorted_key = c->d_key2.as<uint32_t>();
-  c->sorted_val = c->d_val2.as<uint32_t>();
-  p.row_ng = c->sorted_val;
-  const int n_groups = exhaustive ? 1 : (int)std::max<int64_t>(1, std::min<int64_t>(c->pipeline_groups, n_rows >> 16));
-  c->node_kernel_ms_acc = 0;
-  int bg0 = 0, gv0 = vb;
-  const int64_t n_shard_nodes = c->node_end - c->node_begin;
-  // Results outside the shard (filled by lm_tri_import_nodes in a multi-GPU run) start from the empty record, so a
-  // getter never sees uninitialised memory; done once per scene/shard, imports survive later runs.
-  if (!c->outside_shard_clean && (c->node_begin > 0 || c->node_end < c->n_nodes)) {
-    if (c->node_begin > 0) {
-      CU(cudaMemsetAsync(c->d_nodes.p, 0, sizeof(lm::NodeRecord) * c->node_begin, s));
-      CU(cudaMemsetAsync(c->d_node_row_off.p, 0, 4 * c->node_begin, s));
-    }
-    if (c->node_end < c->n_nodes) {
-      CU(cudaMemsetAsync(c->d_nodes.as<lm::NodeRecord>() + c->node_end, 0, sizeof(lm::NodeRecord) * (c->n_nodes - c->node_end), s));
-      CU(cudaMemsetAsync(c->d_node_row_off.as<uint32_t>() + c->node_end + 1, 0, 4 * (c->n_nodes - c->node_end), s));
-    }
-    c->outside_shard_clean = true;
+  c->outside_shard_clean = true;
+  return LM_OK;
+}
+
+static int round_cap(int64_t n, int step) { return (int)std::max<int64_t>(step, (n + step - 1) / step * step); }
+
+// The staging capacity of the node kernel (candidates per node held in shared memory) comes from the previous run
+// (default: 224). A first exhaustive run knows it on the host: every node sees all lines of every neighbour.
+static int initial_cap(const lm_ctx &c, const RunPlan &r, bool fast, int &cap) {
+  const int step = lm::tri_cap_step(fast);
+  cap = c.cap_hint > 0 ? round_cap(c.cap_hint, step) : 224;
+  if (!r.exhaustive || c.cap_hint != 0) return LM_OK;
+  int64_t mr = 0, cur = 0;
+  int cur_src = -1;
+  for (const lm::RawBlock &b : r.blk) {
+    if (b.src_view != cur_src) { cur_src = b.src_view; cur = 0; }
+    cur += c.line_off[b.ng_view + 1] - c.line_off[b.ng_view];
+    mr = std::max(mr, cur);
   }
-  // The staging capacity of the node kernel (candidates per node held in shared memory) comes from the previous run
-  // (default: 224); the kernel flags nodes that do not fit and the run is repeated once with
-  // the exact size. No read-back, no host synchronisation until everything of this run is queued.
-  const bool fast_kernel = lm::tri_fast(p);
-  const size_t smem_limit = (size_t)std::max(0, c->max_smem_optin - 1024);
-  const int cap_step = lm::tri_cap_step(fast_kernel);
-  auto round_cap = [&](int64_t n) { return (int)std::max<int64_t>(cap_step, (n + cap_step - 1) / cap_step * cap_step); };
-  int cap = c->cap_hint > 0 ? round_cap(c->cap_hint) : 224;
-  if (exhaustive && c->cap_hint == 0) { // every node sees all lines of every neighbour: known on the host
-    int64_t mr = 0, cur = 0;
-    int cur_src = -1;
-    for (int i = 0; i < nb; ++i) {
-      if (blk[i].src_view != cur_src) { cur_src = blk[i].src_view; cur = 0; }
-      cur += c->line_off[blk[i].ng_view + 1] - c->line_off[blk[i].ng_view];
-      mr = std::max(mr, cur);
-    }
-    if (mr * ns > 65535) return fail(LM_ERR_INVALID, "more than 65535 candidates possible for one 2D line");
-    cap = round_cap(mr * ns);
+  if (mr * r.ns > 65535) return fail(LM_ERR_INVALID, "more than 65535 candidates possible for one 2D line");
+  cap = round_cap(mr * r.ns, step);
+  return LM_OK;
+}
+
+// First block after pipeline group g, which starts at block b0. Small groups at both ends (smoothstep): the first one is
+// the only one whose matches nothing else can hide, the last one is the only one whose results nothing else can hide.
+// A group finishes its last source image.
+static int group_end(const RunPlan &r, int g, int b0) {
+  if (g + 1 >= r.n_groups) return r.nb;
+  const double tg = (g + 1.0) / r.n_groups;
+  const int64_t target = (int64_t)((double)r.n_rows * (tg * tg * (3.0 - 2.0 * tg)));
+  int b1 = b0;
+  while (b1 < r.nb && r.row_off[b1] < target) ++b1;
+  while (b1 < r.nb && b1 > 0 && r.blk[b1].src_view == r.blk[b1 - 1].src_view) ++b1;
+  return b1;
+}
+
+// Pipeline group g: blocks [b0, b1), source views [v0, v1). The prepare stream waits for the group's matches, expands
+// and sorts its rows and finds every node's rows; the engine's stream runs the node kernel between two timing events;
+// the output stream compacts the group's valid connections and copies its records into the node sink.
+static int queue_group(lm_ctx *c, const RunPlan &r, lm::TriParams p, int g, int b0, int b1, int v0, int v1, Attempt &a) {
+  cudaStream_t s = c->stream, sp = c->prep_stream;
+  const int64_t rb = r.row_off[b0], re = r.row_off[b1];
+  const int64_t node_lo = c->line_off[v0], node_hi = c->line_off[v1];
+  if (!r.exhaustive && re > rb) {
+    int64_t need = 0;
+    for (int b = b0; b < b1; ++b) need = std::max(need, r.blk[b].pair_off + r.blk[b].n_rows);
+    for (const auto &ch : c->chunks) // chunks complete in order: wait for the first one that covers `need`
+      if (ch.row_end >= need) { CU(cudaStreamWaitEvent(sp, ch.ev, 0)); break; }
   }
-  while ((int)c->evk.size() < 2 * n_groups) {
-    cudaEvent_t e;
-    CU(cudaEventCreate(&e));
-    c->evk.push_back(e);
+  if (re > rb) {
+    if (r.exhaustive)
+      lm::launch_expand_exhaustive(c->d_blk_row_off.as<int64_t>(), c->d_blk_src.as<int32_t>(), c->d_blk_ng.as<int32_t>(),
+                                   r.nb, c->d_line_off.as<int64_t>(), r.n_rows, c->d_key.as<uint32_t>(),
+                                   c->d_val.as<uint32_t>(), sp);
+    else
+      lm::launch_expand_rows(c->d_pairs.as<int32_t>(), c->d_blk_row_off.as<int64_t>(), c->d_blk_src.as<int32_t>(),
+                             c->d_blk_ng.as<int32_t>(), c->d_blk_pair_off.as<int64_t>(), r.nb,
+                             c->d_line_off.as<int64_t>(), rb, re, c->d_key.as<uint32_t>(), c->d_val.as<uint32_t>(),
+                             c->d_scalars.as<int>() + 1, sp);
+    ++a.launches;
+    // stable LSD radix sort by node id keeps (neighbour, row) order inside every node
+    cub::DoubleBuffer<uint32_t> dk(c->d_key.as<uint32_t>() + rb, c->d_key2.as<uint32_t>() + rb);
+    cub::DoubleBuffer<uint32_t> dv(c->d_val.as<uint32_t>() + rb, c->d_val2.as<uint32_t>() + rb);
+    CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, dk, dv, (int)(re - rb), 0, r.node_bits, sp);
+    }));
+    a.launches += (r.node_bits + 7) / 8 + 1;
+    if (dk.Current() != c->d_key2.as<uint32_t>() + rb) {
+      CU(cudaMemcpyAsync(c->d_key2.as<uint32_t>() + rb, dk.Current(), 4 * (re - rb), cudaMemcpyDeviceToDevice, sp));
+      CU(cudaMemcpyAsync(c->d_val2.as<uint32_t>() + rb, dv.Current(), 4 * (re - rb), cudaMemcpyDeviceToDevice, sp));
+    }
   }
-  while ((int)c->evp.size() < n_groups) {
-    cudaEvent_t e;
-    CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    c->evp.push_back(e);
+  lm::launch_node_offsets(c->sorted_key + rb, re - rb, rb, node_lo, node_hi, c->d_node_row_off.as<uint32_t>(),
+                          c->d_scalars.as<unsigned int>() + 16 + g, sp);
+  ++a.launches;
+  CU(cudaEventRecord(c->evp[g], sp));
+  CU(cudaStreamWaitEvent(s, c->evp[g], 0));
+  p.node_begin = node_lo; p.node_end = node_hi; p.cap = a.cap;
+  const int64_t n_group_nodes = node_hi - node_lo;
+  size_t smem = lm::tri_smem_bytes(a.cap, a.fast);
+  int grid;
+  if (smem <= (size_t)std::max(0, c->max_smem_optin - 1024)) {
+    p.use_slab = 0;
+    grid = (int)std::min<int64_t>(n_group_nodes, (int64_t)1 << 30);
+  } else {
+    // nodes larger than shared memory (exhaustive matching): persistent CTAs with a global staging slab
+    p.use_slab = 1;
+    grid = (int)std::min<int64_t>(n_group_nodes, (int64_t)c->sm_count * 4);
+    p.slab_stride = (int64_t)((smem + 255) / 256 * 256);
+    CU(c->d_slab.ensure((size_t)p.slab_stride * std::max(grid, 1)));
+    p.slab = c->d_slab.as<char>();
+    smem = 0;
   }
-  std::vector<int> group_has_kernel(n_groups, 0);
-  CU(c->d_nvalid.ensure(4 * (n_shard_nodes + 2)));
-  CU(c->d_local_off.ensure(4 * (n_shard_nodes + 2)));
-  CU(c->d_edge_off.ensure(4 * (n_shard_nodes + 2)));
-  CU(c->d_edge_ng.ensure(4 * std::max<int64_t>(n_rows * ns, 1)));
-  for (int g = 0; g < n_groups; ++g) {
-    // blocks [bg0, bg1) with whole source images, views [gv0, gv1)
-    int bg1 = nb, gv1 = ve;
-    if (g + 1 < n_groups) {
-      // small groups at both ends (smoothstep): the first one is the only one whose matches nothing else can hide, the
-      // last one is the only one whose results nothing else can hide
-      const double tg = (g + 1.0) / n_groups;
-      const int64_t target = (int64_t)((double)n_rows * (tg * tg * (3.0 - 2.0 * tg)));
-      bg1 = bg0;
-      while (bg1 < nb && row_off[bg1] < target) ++bg1;
-      while (bg1 < nb && bg1 > 0 && blk[bg1].src_view == blk[bg1 - 1].src_view) ++bg1; // finish the image
-      gv1 = (bg1 < nb) ? blk[bg1].src_view : ve;
-    }
-    const int64_t rb = row_off[bg0], re = row_off[bg1];
-    const int64_t node_lo = c->line_off[gv0], node_hi = c->line_off[gv1];
-    if (!exhaustive && re > rb) {
-      int64_t need = 0;
-      for (int b2 = bg0; b2 < bg1; ++b2) need = std::max(need, pair_off[b2] + blk[b2].n_rows);
-      for (const auto &ch : c->chunks) // chunks complete in order: wait for the first one that covers `need`
-        if (ch.row_end >= need) { CU(cudaStreamWaitEvent(sp, ch.ev, 0)); break; }
-    }
-    unsigned int *d_max_rows = c->d_scalars.as<unsigned int>() + 16 + g;
-    if (re > rb) {
-      if (exhaustive)
-        lm::launch_expand_exhaustive(c->d_blk_row_off.as<int64_t>(), c->d_blk_src.as<int32_t>(), c->d_blk_ng.as<int32_t>(),
-                                     nb, c->d_line_off.as<int64_t>(), n_rows, c->d_key.as<uint32_t>(),
-                                     c->d_val.as<uint32_t>(), sp);
-      else
-        lm::launch_expand_rows(c->d_pairs.as<int32_t>(), c->d_blk_row_off.as<int64_t>(), c->d_blk_src.as<int32_t>(),
-                               c->d_blk_ng.as<int32_t>(), c->d_blk_pair_off.as<int64_t>(), nb,
-                               c->d_line_off.as<int64_t>(), rb, re, c->d_key.as<uint32_t>(), c->d_val.as<uint32_t>(),
-                               d_err, sp);
-      ++launches;
-      // stable LSD radix sort by node id keeps (neighbour, row) order inside every node
-      cub::DoubleBuffer<uint32_t> dk(c->d_key.as<uint32_t>() + rb, c->d_key2.as<uint32_t>() + rb);
-      cub::DoubleBuffer<uint32_t> dv(c->d_val.as<uint32_t>() + rb, c->d_val2.as<uint32_t>() + rb);
-      CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) {
-        return cub::DeviceRadixSort::SortPairs(t, b, dk, dv, (int)(re - rb), 0, nbits, sp);
-      }));
-      launches += (nbits + 7) / 8 + 1;
-      if (dk.Current() != c->d_key2.as<uint32_t>() + rb) {
-        CU(cudaMemcpyAsync(c->d_key2.as<uint32_t>() + rb, dk.Current(), 4 * (re - rb), cudaMemcpyDeviceToDevice, sp));
-        CU(cudaMemcpyAsync(c->d_val2.as<uint32_t>() + rb, dv.Current(), 4 * (re - rb), cudaMemcpyDeviceToDevice, sp));
-      }
-    }
-    lm::launch_node_offsets(c->sorted_key + rb, re - rb, rb, node_lo, node_hi, c->d_node_row_off.as<uint32_t>(),
-                            d_max_rows, sp);
-    ++launches;
-    CU(cudaEventRecord(c->evp[g], sp));
-    CU(cudaStreamWaitEvent(s, c->evp[g], 0));
-    p.node_begin = node_lo;
-    p.node_end = node_hi;
-    const int64_t n_group_nodes = node_hi - node_lo;
-    size_t smem = lm::tri_smem_bytes(cap, fast_kernel);
-    int grid;
-    if (smem <= smem_limit) {
-      p.use_slab = 0;
-      p.cap = cap;
-      grid = (int)std::min<int64_t>(n_group_nodes, (int64_t)1 << 30);
-    } else {
-      // nodes larger than shared memory (exhaustive matching): persistent CTAs with a global staging slab
-      p.use_slab = 1;
-      p.cap = cap;
-      grid = (int)std::min<int64_t>(n_group_nodes, (int64_t)c->sm_count * 4);
-      p.slab_stride = (int64_t)((smem + 255) / 256 * 256);
-      CU(c->d_slab.ensure((size_t)p.slab_stride * std::max(grid, 1)));
-      p.slab = c->d_slab.as<char>();
-      smem = 0;
-    }
-    if (n_group_nodes > 0) {
-      CU(cudaEventRecord(c->evk[2 * g], s));
-      CU(lm::launch_tri_node_kernel(p, grid, smem, s));
-      CU(cudaEventRecord(c->evk[2 * g + 1], s));
-      group_has_kernel[g] = 1;
-      ++launches;
-      // valid_edges_ of the group in compact form: per-node counts -> exclusive scan -> ordered scatter at the global
-      // offsets
-      {
-        cudaStream_t so = c->out_stream; // under the node kernels of the later groups
-        CU(cudaStreamWaitEvent(so, c->evk[2 * g + 1], 0));
-        uint32_t *nv = c->d_nvalid.as<uint32_t>() + (node_lo - c->node_begin);
-        lm::launch_extract_nvalid(p.nodes, node_lo, n_group_nodes, nv, so);
-        // (d_scan_tmp, not d_sort_tmp: the preparation stream sorts the next group meanwhile)
-        CU(cub_call(c->d_scan_tmp, [&](void *t, size_t &b) {
-          return cub::DeviceScan::ExclusiveSum(t, b, nv, c->d_local_off.as<uint32_t>(), (int)(n_group_nodes + 1), so);
-        }));
-        lm::launch_group_edges(p.row_state, p.row_ng, p.node_row_off, c->d_local_off.as<uint32_t>(),
-                               c->d_scalars.as<unsigned int>() + 80, g, c->node_begin, node_lo, n_group_nodes, ns,
-                               c->d_edge_off.as<uint32_t>(), c->d_edge_ng.as<uint32_t>(), so);
-        launches += 4;
-      }
-      if (c->node_sink) { // the group's records go to the caller's buffer under the kernels of the later groups
-        CU(cudaMemcpyAsync(c->node_sink + sizeof(lm::NodeRecord) * node_lo, c->d_nodes.as<lm::NodeRecord>() + node_lo,
-                           sizeof(lm::NodeRecord) * n_group_nodes, cudaMemcpyDeviceToHost, c->out_stream));
-      }
-    }
-    bg0 = bg1;
-    gv0 = gv1;
-  }
-  p.node_begin = c->node_begin;
-  p.node_end = c->node_end;
+  if (n_group_nodes <= 0) return LM_OK;
+  CU(cudaEventRecord(c->evk[2 * g], s));
+  CU(lm::launch_tri_node_kernel(p, grid, smem, s));
+  CU(cudaEventRecord(c->evk[2 * g + 1], s));
+  a.group_has_kernel[g] = 1;
+  ++a.launches;
+  // valid_edges_ of the group in compact form, under the node kernels of the later groups: per-node counts -> exclusive
+  // scan -> ordered scatter at the global offsets
+  cudaStream_t so = c->out_stream;
+  CU(cudaStreamWaitEvent(so, c->evk[2 * g + 1], 0));
+  uint32_t *nv = c->d_nvalid.as<uint32_t>() + (node_lo - c->node_begin);
+  lm::launch_extract_nvalid(p.nodes, node_lo, n_group_nodes, nv, so);
+  // (d_scan_tmp, not d_sort_tmp: the preparation stream sorts the next group meanwhile)
+  CU(cub_call(c->d_scan_tmp, [&](void *t, size_t &b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, nv, c->d_local_off.as<uint32_t>(), (int)(n_group_nodes + 1), so);
+  }));
+  lm::launch_group_edges(p.row_state, p.row_ng, p.node_row_off, c->d_local_off.as<uint32_t>(),
+                         c->d_scalars.as<unsigned int>() + 80, g, c->node_begin, node_lo, n_group_nodes, r.ns,
+                         c->d_edge_off.as<uint32_t>(), c->d_edge_ng.as<uint32_t>(), so);
+  a.launches += 4;
+  if (c->node_sink) // the group's records go to the caller's buffer under the kernels of the later groups
+    CU(cudaMemcpyAsync(c->node_sink + sizeof(lm::NodeRecord) * node_lo, c->d_nodes.as<lm::NodeRecord>() + node_lo,
+                       sizeof(lm::NodeRecord) * n_group_nodes, cudaMemcpyDeviceToHost, c->out_stream));
+  return LM_OK;
+}
+
+// The end of an attempt: the engine's stream waits for the output stream, then the one read-back of the run (error and
+// overflow flags, counters, largest node per group) and its one host synchronisation. Sets `overflow` when some node did
+// not fit the staging capacity: the hint is then exact, and the stats are left to the repeated attempt.
+static int finish_run(lm_ctx *c, const RunPlan &r, const Attempt &a, bool &overflow) {
+  cudaStream_t s = c->stream;
   CU(cudaGetLastError());
   // the engine's stream ends the run: whatever follows on it (getters, exchange) sees the compact connections
   CU(cudaEventRecord(c->ev_run_begin, c->out_stream));
   CU(cudaStreamWaitEvent(s, c->ev_run_begin, 0));
   CU(cudaEventRecord(c->ev1, s));
-  // one read-back for the whole run: error / overflow flags, counters, largest node per group
-  unsigned int *hs = c->h_pin;
-  CU(cudaMemcpyAsync(hs, c->d_scalars.p, 512, cudaMemcpyDeviceToHost, s));
+  const unsigned int *hs = c->h_pin;
+  CU(cudaMemcpyAsync(c->h_pin, c->d_scalars.p, 512, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   CU(cudaStreamSynchronize(c->copy_stream)); // uploads of images outside this shard may still be in flight
   CU(cudaStreamSynchronize(c->out_stream));
-  c->stats.n_kernel_launches += launches;
+  c->stats.n_kernel_launches += a.launches;
   if (hs[1] == 1)
     return fail(LM_ERR_INVALID, "IndexError! Out-of-index matches exist (line_id >= number of lines of the image). "
                                 "Please make sure you are reusing the correct descriptors and matches.");
   if (hs[1] == 2) return fail(LM_ERR_INVALID, "IndexError! Out-of-index neighbor line id in matches.");
   int max_rows_all = 0;
-  for (int g = 0; g < n_groups; ++g) max_rows_all = std::max(max_rows_all, (int)hs[16 + g]);
-  if ((int64_t)max_rows_all * ns > 65535) return fail(LM_ERR_INVALID, "more than 65535 candidates possible for one 2D line");
-  c->cap_hint = round_cap((int64_t)max_rows_all * ns);
-  if (hs[2] != 0) { // some node did not fit the staging area sized from the hint: repeat with the exact size
-    if (c->run_retry) { c->run_retry = 0; return fail(LM_ERR_STATE, "node staging overflow after resizing"); }
-    c->run_retry = 1;
-    const int rc2 = lm_tri_run(c);
-    c->run_retry = 0;
-    return rc2;
-  }
+  for (int g = 0; g < r.n_groups; ++g) max_rows_all = std::max(max_rows_all, (int)hs[16 + g]);
+  if ((int64_t)max_rows_all * r.ns > 65535) return fail(LM_ERR_INVALID, "more than 65535 candidates possible for one 2D line");
+  c->cap_hint = round_cap((int64_t)max_rows_all * r.ns, lm::tri_cap_step(a.fast));
+  overflow = hs[2] != 0;
+  if (overflow) return LM_OK;
   float ms = 0;
   CU(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-  for (int g = 0; g < n_groups; ++g)
-    if (group_has_kernel[g]) {
+  double node_kernel_ms = 0;
+  for (int g = 0; g < r.n_groups; ++g)
+    if (a.group_has_kernel[g]) {
       float msk = 0;
       CU(cudaEventElapsedTime(&msk, c->evk[2 * g], c->evk[2 * g + 1]));
-      c->node_kernel_ms_acc += msk;
+      node_kernel_ms += msk;
     }
   c->stats.max_rows_per_node = max_rows_all;
-  c->stats.last_node_kernel_ms = c->node_kernel_ms_acc;
+  c->stats.last_node_kernel_ms = node_kernel_ms;
   const unsigned long long *cnt = reinterpret_cast<const unsigned long long *>(hs + 4);
-  c->stats.n_rows = n_rows;
+  c->stats.n_rows = r.n_rows;
   c->stats.n_candidates = (int64_t)cnt[0];
   c->stats.n_valid_edges = (int64_t)cnt[1];
   c->stats.n_pairs_gated = (int64_t)cnt[2];
@@ -913,6 +868,60 @@ int lm_tri_run(lm_ctx *c) {
   c->stats.last_run_ms = ms;
   c->ran = true;
   return LM_OK;
+}
+
+int lm_tri_run(lm_ctx *c) {
+  if (!c) return fail(LM_ERR_INVALID, "ctx is NULL");
+  if (!c->have_scene) return fail(LM_ERR_STATE, "no scene uploaded");
+  if (!c->have_cfg) return fail(LM_ERR_STATE, "lm_tri_configure must precede lm_tri_run");
+  CU(cudaSetDevice(c->device));
+  RunPlan plan;
+  int rc = plan_run(*c, plan);
+  if (rc) return rc;
+  c->n_rows = plan.n_rows;
+  c->ns = plan.ns;
+  c->node_begin = c->line_off[plan.vb];
+  c->node_end = c->line_off[plan.ve];
+  c->h_nodes_valid = c->h_rows_valid = c->h_edges_valid = false;
+  c->edges_collected = c->edges_count_on_device = false;
+  c->tracks.clear();
+  if ((rc = ensure_run_buffers(c, plan))) return rc;
+  // canonical sorted buffers: d_key2 / d_val2
+  c->sorted_key = c->d_key2.as<uint32_t>();
+  c->sorted_val = c->d_val2.as<uint32_t>();
+  const lm::TriParams p = make_tri_params(*c, plan.ns);
+  // Two compute streams: `sp` prepares the rows of a pipeline group (expansion, sort, node offsets), `s` runs the node
+  // kernels. The preparation of group g+1 is queued right behind that of group g, so it executes under the node kernel of
+  // group g; everything `sp` touches is per-group slices, its own scratch, or is read by `s` only after the group's event.
+  cudaStream_t s = c->stream, sp = c->prep_stream;
+  // The kernel flags the nodes that do not fit the staging capacity, and the run is then repeated once at the exact
+  // size. No read-back, no host synchronisation until everything of an attempt is queued.
+  for (int attempt = 0;; ++attempt) {
+    CU(cudaEventRecord(c->ev0, s));
+    CU(cudaEventRecord(c->ev_run_begin, s)); // whatever the caller queued on the engine's stream comes first
+    CU(cudaStreamWaitEvent(sp, c->ev_run_begin, 0));
+    // scene tables / VP tables travel on the copy stream (see lm_ctx::ev_scene)
+    CU(cudaStreamWaitEvent(sp, c->ev_scene, 0));
+    CU(cudaStreamWaitEvent(s, c->ev_scene, 0));
+    lm::launch_zero_words(c->d_scalars.p, 256, sp);
+    if ((rc = queue_block_tables(c, plan))) return rc;
+    if ((rc = clear_outside_shard(c))) return rc;
+    Attempt a;
+    a.fast = lm::tri_fast(p);
+    if ((rc = initial_cap(*c, plan, a.fast, a.cap))) return rc;
+    a.group_has_kernel.assign(plan.n_groups, 0);
+    // groups of whole source images: sort + node kernel of group g overlap the upload of group g+1
+    for (int g = 0, b0 = 0, v0 = plan.vb; g < plan.n_groups; ++g) {
+      const int b1 = group_end(plan, g, b0), v1 = (b1 < plan.nb) ? plan.blk[b1].src_view : plan.ve;
+      if ((rc = queue_group(c, plan, p, g, b0, b1, v0, v1, a))) return rc;
+      b0 = b1;
+      v0 = v1;
+    }
+    bool overflow = false;
+    if ((rc = finish_run(c, plan, a, overflow))) return rc;
+    if (!overflow) return LM_OK;
+    if (attempt > 0) return fail(LM_ERR_STATE, "node staging overflow after resizing");
+  }
 }
 
 int lm_tri_get_stats(lm_ctx *c, lm_tri_stats *out) {

@@ -74,13 +74,6 @@ template <typename F> cudaError_t cub_call(DevBuf &scratch, F f) {
   return e;
 }
 
-struct MatchBlock {
-  int src_view, ng_view;
-  int64_t n_rows;
-  int64_t pair_off; // row offset into the device pairs store (-1: exhaustive)
-  int order;        // insertion order within the source image (exhaustive mode keeps the given order)
-};
-
 struct M3h {
   double m[9];
 };
@@ -133,7 +126,6 @@ struct lm_ctx {
   struct CopyChunk { int64_t row_end; cudaEvent_t ev; };
   std::vector<CopyChunk> chunks;
   std::vector<cudaEvent_t> event_pool;
-  double node_kernel_ms_acc = 0;
   DevBuf d_raw_blocks, d_bkey, d_bkey2, d_bval, d_bval2, d_blk_rows; // device mirror of `blocks` + sort scratch
   int64_t raw_uploaded = 0;
   cudaEvent_t ev_raw = nullptr; // recorded on the copy stream after the latest descriptor upload
@@ -150,7 +142,6 @@ struct lm_ctx {
   bool edges_count_on_device = false; // n_edges_dev is still on the device (lm_tri_unpack_messages)
   int cap_hint = 0;                  // staging capacity of the node kernel, from the previous run (0: default)
   bool outside_shard_clean = false;  // node records / row offsets outside the shard were zero-filled
-  int run_retry = 0;
   int sm_count = 132;
   int max_smem_optin = 0;
   // scene
@@ -171,9 +162,8 @@ struct lm_ctx {
   DevBuf d_vp_label, d_vp_voff, d_vp_vps;
   int ns = 1; // proposal slots per match row of the last run (3 with VP proposals)
   // staged matches
-  std::vector<MatchBlock> blocks;
+  std::vector<lm::RawBlock> blocks; // one per (source image, neighbour) table, in the order they were added
   std::vector<char> image_added;
-  std::vector<int> image_norder;
   DevBuf d_pairs;
   int64_t pairs_rows = 0;
   bool any_exhaustive = false, any_matches = false;
