@@ -67,7 +67,7 @@ static int fetch_rows(lm_ctx *c) {
   CU(cudaMemcpyAsync(c->h_node_row_off.data(), c->d_node_row_off.p, 4 * (c->n_nodes + 1), cudaMemcpyDeviceToHost,
                      c->stream));
   if (c->n_rows) {
-    CU(cudaMemcpyAsync(c->h_row_ng.data(), c->sorted_val, 4 * c->n_rows, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(c->h_row_ng.data(), c->d_row_ng.p, 4 * c->n_rows, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaMemcpyAsync(c->h_row_state.data(), c->d_row_state.p, c->n_rows * c->ns, cudaMemcpyDeviceToHost, c->stream));
     if (c->cfg.debug_mode) {
       c->h_row_cand.resize(c->n_rows * c->ns * 10);
@@ -544,7 +544,8 @@ struct RunPlan {
   std::vector<int64_t> row_off;  // first flat row of every block; row_off[nb] = n_rows
   int nb = 0, n_groups = 1;      // blocks, pipeline groups
   int64_t n_rows = 0;
-  int node_bits = 1;             // key bits of the row sort by node id
+  std::vector<int64_t> chunk_off; // first row chunk (lm::kRowChunk rows) of every block; chunk_off[nb] = chunks
+  std::vector<int64_t> tab_off;   // [V+1] first count-table entry of every view of the shard (lines x chunks)
 };
 
 // What one attempt of the run queued (a staging overflow repeats the run once): whether tri_node_kernel's fast
@@ -576,7 +577,17 @@ static int plan_run(const lm_ctx &c, RunPlan &r) {
   // the sort and scan item counts are 32-bit signed
   if (r.n_rows >= ((int64_t)1 << 31) - 64) return fail(LM_ERR_INVALID, "more than 2^31 match rows in one run (shard the scene by source image)");
   r.n_groups = r.exhaustive ? 1 : (int)std::max<int64_t>(1, std::min<int64_t>(c.pipeline_groups, r.n_rows >> 16));
-  while (((int64_t)1 << r.node_bits) < c.n_nodes) ++r.node_bits;
+  // the sizes of the chunk and count tables that queue_block_tables derives on the device
+  r.chunk_off.assign(r.nb + 1, 0);
+  for (int i = 0; i < r.nb; ++i) r.chunk_off[i + 1] = r.chunk_off[i] + (r.blk[i].n_rows + lm::kRowChunk - 1) / lm::kRowChunk;
+  r.tab_off.assign(c.V + 1, 0);
+  for (int v = r.vb, i = 0; v < r.ve; ++v) {
+    const int64_t k = r.chunk_off[i];
+    while (i < r.nb && r.blk[i].src_view == v) ++i;
+    r.tab_off[v + 1] = r.tab_off[v] + (c.line_off[v + 1] - c.line_off[v]) * (r.chunk_off[i] - k);
+  }
+  if (r.tab_off[r.ve] >= ((int64_t)1 << 31) - 64)
+    return fail(LM_ERR_INVALID, "more than 2^31 (line, row chunk) counts in one run (shard the scene by source image)");
   return LM_OK;
 }
 
@@ -589,8 +600,14 @@ static int ensure_run_buffers(lm_ctx *c, const RunPlan &r) {
   CU(c->d_blk_src.ensure(4 * std::max(nb + 1, 2)));
   CU(c->d_blk_ng.ensure(4 * std::max(nb + 1, 2)));
   CU(c->d_blk_pair_off.ensure(8 * std::max(nb, 1)));
-  CU(c->d_key.ensure(4 * rows)); CU(c->d_key2.ensure(4 * rows));
-  CU(c->d_val.ensure(4 * rows)); CU(c->d_val2.ensure(4 * rows));
+  CU(c->d_row_ng.ensure(4 * rows));
+  CU(c->d_blk_chunks.ensure(4 * (nb + 2))); CU(c->d_blk_chunk_off.ensure(4 * (nb + 2)));
+  CU(c->d_view_chunk_off.ensure(4 * (c->V + 1))); CU(c->d_view_ent.ensure(4 * (c->V + 1)));
+  CU(c->d_view_tab_off.ensure(4 * (c->V + 1))); CU(c->d_view_row_off.ensure(8 * (c->V + 1)));
+  if (!r.exhaustive) {
+    const int64_t ent = std::max<int64_t>(r.tab_off[r.ve], 1);
+    CU(c->d_row_cnt.ensure(2 * ent)); CU(c->d_row_pos.ensure(4 * ent));
+  }
   CU(c->d_node_row_off.ensure(4 * (c->n_nodes + 2)));
   CU(c->d_scalars.ensure(1024));
   CU(c->d_nodes.ensure(sizeof(lm::NodeRecord) * std::max<int64_t>(c->n_nodes, 1)));
@@ -611,7 +628,23 @@ static int ensure_run_buffers(lm_ctx *c, const RunPlan &r) {
 }
 
 // The shard's block tables, derived on the prepare stream from the descriptors uploaded with the matches (no transfer
-// now): keys by (source view, neighbour order), CUB sort, gather, and the exclusive scan of the rows.
+// now): keys by (source view, neighbour order), CUB sort, gather, the exclusive scans of the rows and row chunks, and
+// the per-view chunk, row and count-table offsets.
+static lm::RowTables row_tables(const lm_ctx &c, const RunPlan &r) {
+  lm::RowTables t;
+  t.blk_row_off = c.d_blk_row_off.as<int64_t>();
+  t.blk_src = c.d_blk_src.as<int32_t>();
+  t.blk_ng = c.d_blk_ng.as<int32_t>();
+  t.blk_pair_off = c.d_blk_pair_off.as<int64_t>();
+  t.blk_chunk_off = c.d_blk_chunk_off.as<int32_t>();
+  t.nb = r.nb;
+  t.line_off = c.d_line_off.as<int64_t>();
+  t.view_chunk_off = c.d_view_chunk_off.as<int32_t>();
+  t.view_tab_off = c.d_view_tab_off.as<int32_t>();
+  t.view_row_off = c.d_view_row_off.as<int64_t>();
+  return t;
+}
+
 static int queue_block_tables(lm_ctx *c, const RunPlan &r) {
   cudaStream_t sp = c->prep_stream;
   const int nb = r.nb, n_all = (int)c->blocks.size();
@@ -624,12 +657,23 @@ static int queue_block_tables(lm_ctx *c, const RunPlan &r) {
     cub::DoubleBuffer<uint32_t> bv(c->d_bval.as<uint32_t>(), c->d_bval2.as<uint32_t>());
     CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, bk, bv, n_all, 0, 32, sp); }));
     lm::launch_block_gather(c->d_raw_blocks.as<lm::RawBlock>(), bv.Current(), nb, c->d_blk_src.as<int32_t>(),
-                            c->d_blk_ng.as<int32_t>(), c->d_blk_pair_off.as<int64_t>(), c->d_blk_rows.as<int64_t>(), sp);
+                            c->d_blk_ng.as<int32_t>(), c->d_blk_pair_off.as<int64_t>(), c->d_blk_rows.as<int64_t>(),
+                            c->d_blk_chunks.as<int32_t>(), sp);
   } else {
     lm::launch_zero_words(c->d_blk_rows.p, 4, sp);
+    lm::launch_zero_words(c->d_blk_chunks.p, 2, sp);
   }
   CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) {
     return cub::DeviceScan::ExclusiveSum(t, b, c->d_blk_rows.as<int64_t>(), c->d_blk_row_off.as<int64_t>(), nb + 1, sp);
+  }));
+  CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, c->d_blk_chunks.as<int32_t>(), c->d_blk_chunk_off.as<int32_t>(), nb + 1, sp);
+  }));
+  const lm::RowTables t = row_tables(*c, r);
+  int32_t *ent = c->d_view_ent.as<int32_t>();
+  lm::launch_view_tables(t, r.vb, r.ve, ent, sp);
+  CU(cub_call(c->d_sort_tmp, [&](void *tmp, size_t &b) {
+    return cub::DeviceScan::ExclusiveSum(tmp, b, ent + r.vb, c->d_view_tab_off.as<int32_t>() + r.vb, r.ve - r.vb + 1, sp);
   }));
   return LM_OK;
 }
@@ -647,7 +691,7 @@ static lm::TriParams make_tri_params(const lm_ctx &c, int ns) {
   p.nodes = c.d_nodes.as<lm::NodeRecord>();
   p.row_state = c.d_row_state.as<uint8_t>();
   p.row_cand = c.cfg.debug_mode ? c.d_row_cand.as<double>() : nullptr;
-  p.row_ng = c.sorted_val;
+  p.row_ng = c.d_row_ng.as<uint32_t>();
   // d_scalars words: [1] index error, [2] staging overflow, bytes 16..47 counters, words [16 + g] largest node of group g
   p.counters = reinterpret_cast<unsigned long long *>(c.d_scalars.as<char>() + 16);
   p.overflow = c.d_scalars.as<int>() + 2;
@@ -740,8 +784,8 @@ static int group_end(const RunPlan &r, int g, int b0) {
   return b1;
 }
 
-// Pipeline group g: blocks [b0, b1), source views [v0, v1). The prepare stream waits for the group's matches, expands
-// and sorts its rows and finds every node's rows; the engine's stream runs the node kernel between two timing events;
+// Pipeline group g: blocks [b0, b1), source views [v0, v1). The prepare stream waits for the group's matches, puts its
+// rows in node order and finds every node's rows; the engine's stream runs the node kernel between two timing events;
 // the output stream compacts the group's valid connections and copies its records into the node sink.
 static int queue_group(lm_ctx *c, const RunPlan &r, lm::TriParams p, int g, int b0, int b1, int v0, int v1, Attempt &a) {
   cudaStream_t s = c->stream, sp = c->prep_stream;
@@ -753,32 +797,34 @@ static int queue_group(lm_ctx *c, const RunPlan &r, lm::TriParams p, int g, int 
     for (const auto &ch : c->chunks) // chunks complete in order: wait for the first one that covers `need`
       if (ch.row_end >= need) { CU(cudaStreamWaitEvent(sp, ch.ev, 0)); break; }
   }
+  // rows in node order (tri_plumbing.cu): matches count the rows of every (line, row chunk), scan the group's slice of
+  // the count table and place every chunk's rows; exhaustive matching places every row in closed form
+  const lm::RowTables t = row_tables(*c, r);
+  uint32_t *row_ng = c->d_row_ng.as<uint32_t>();
+  const uint32_t *pos = c->d_row_pos.as<uint32_t>();
+  const int k0 = (int)r.chunk_off[b0], n_chunks = (int)(r.chunk_off[b1] - r.chunk_off[b0]);
+  const int64_t t0 = r.tab_off[v0], t1 = r.tab_off[v1];
+  int nl_max = 0;
+  for (int v = v0; v < v1; ++v) nl_max = std::max(nl_max, (int)(c->line_off[v + 1] - c->line_off[v]));
+  if (re > rb && !r.exhaustive) {
+    CU(lm::launch_row_count(t, c->d_pairs.as<int32_t>(), k0, n_chunks, nl_max, c->d_row_cnt.as<uint16_t>(),
+                            c->d_scalars.as<int>() + 1, sp));
+    CU(cub_call(c->d_sort_tmp, [&](void *tmp, size_t &b) {
+      return cub::DeviceScan::ExclusiveScan(tmp, b, c->d_row_cnt.as<uint16_t>() + t0, c->d_row_pos.as<uint32_t>() + t0,
+                                            ::cuda::std::plus<uint32_t>(), (uint32_t)0, (int)(t1 - t0), sp);
+    }));
+    a.launches += 3; // count, the scan's two kernels
+  }
+  lm::launch_node_row_off(t, pos, t1, rb, re, node_lo, node_hi, c->V, r.exhaustive ? 1 : 0,
+                          c->d_node_row_off.as<uint32_t>(), c->d_scalars.as<unsigned int>() + 16 + g, sp);
+  ++a.launches;
   if (re > rb) {
     if (r.exhaustive)
-      lm::launch_expand_exhaustive(c->d_blk_row_off.as<int64_t>(), c->d_blk_src.as<int32_t>(), c->d_blk_ng.as<int32_t>(),
-                                   r.nb, c->d_line_off.as<int64_t>(), r.n_rows, c->d_key.as<uint32_t>(),
-                                   c->d_val.as<uint32_t>(), sp);
+      lm::launch_place_exhaustive(t, r.n_rows, row_ng, sp);
     else
-      lm::launch_expand_rows(c->d_pairs.as<int32_t>(), c->d_blk_row_off.as<int64_t>(), c->d_blk_src.as<int32_t>(),
-                             c->d_blk_ng.as<int32_t>(), c->d_blk_pair_off.as<int64_t>(), r.nb,
-                             c->d_line_off.as<int64_t>(), rb, re, c->d_key.as<uint32_t>(), c->d_val.as<uint32_t>(),
-                             c->d_scalars.as<int>() + 1, sp);
+      CU(lm::launch_row_place(t, c->d_pairs.as<int32_t>(), k0, n_chunks, nl_max, pos, rb, row_ng, sp));
     ++a.launches;
-    // stable LSD radix sort by node id keeps (neighbour, row) order inside every node
-    cub::DoubleBuffer<uint32_t> dk(c->d_key.as<uint32_t>() + rb, c->d_key2.as<uint32_t>() + rb);
-    cub::DoubleBuffer<uint32_t> dv(c->d_val.as<uint32_t>() + rb, c->d_val2.as<uint32_t>() + rb);
-    CU(cub_call(c->d_sort_tmp, [&](void *t, size_t &b) {
-      return cub::DeviceRadixSort::SortPairs(t, b, dk, dv, (int)(re - rb), 0, r.node_bits, sp);
-    }));
-    a.launches += (r.node_bits + 7) / 8 + 1;
-    if (dk.Current() != c->d_key2.as<uint32_t>() + rb) {
-      CU(cudaMemcpyAsync(c->d_key2.as<uint32_t>() + rb, dk.Current(), 4 * (re - rb), cudaMemcpyDeviceToDevice, sp));
-      CU(cudaMemcpyAsync(c->d_val2.as<uint32_t>() + rb, dv.Current(), 4 * (re - rb), cudaMemcpyDeviceToDevice, sp));
-    }
   }
-  lm::launch_node_offsets(c->sorted_key + rb, re - rb, rb, node_lo, node_hi, c->d_node_row_off.as<uint32_t>(),
-                          c->d_scalars.as<unsigned int>() + 16 + g, sp);
-  ++a.launches;
   CU(cudaEventRecord(c->evp[g], sp));
   CU(cudaStreamWaitEvent(s, c->evp[g], 0));
   p.node_begin = node_lo; p.node_end = node_hi; p.cap = a.cap;
@@ -809,7 +855,7 @@ static int queue_group(lm_ctx *c, const RunPlan &r, lm::TriParams p, int g, int 
   CU(cudaStreamWaitEvent(so, c->evk[2 * g + 1], 0));
   uint32_t *nv = c->d_nvalid.as<uint32_t>() + (node_lo - c->node_begin);
   lm::launch_extract_nvalid(p.nodes, node_lo, n_group_nodes, nv, so);
-  // (d_scan_tmp, not d_sort_tmp: the preparation stream sorts the next group meanwhile)
+  // (d_scan_tmp, not d_sort_tmp: the preparation stream scans the next group's counts meanwhile)
   CU(cub_call(c->d_scan_tmp, [&](void *t, size_t &b) {
     return cub::DeviceScan::ExclusiveSum(t, b, nv, c->d_local_off.as<uint32_t>(), (int)(n_group_nodes + 1), so);
   }));
@@ -887,11 +933,8 @@ int lm_tri_run(lm_ctx *c) {
   c->edges_collected = c->edges_count_on_device = c->edges_overflowed = false;
   c->tracks.clear();
   if ((rc = ensure_run_buffers(c, plan))) return rc;
-  // canonical sorted buffers: d_key2 / d_val2
-  c->sorted_key = c->d_key2.as<uint32_t>();
-  c->sorted_val = c->d_val2.as<uint32_t>();
   const lm::TriParams p = make_tri_params(*c, plan.ns);
-  // Two compute streams: `sp` prepares the rows of a pipeline group (expansion, sort, node offsets), `s` runs the node
+  // Two compute streams: `sp` prepares the rows of a pipeline group (node order, node offsets), `s` runs the node
   // kernels. The preparation of group g+1 is queued right behind that of group g, so it executes under the node kernel of
   // group g; everything `sp` touches is per-group slices, its own scratch, or is read by `s` only after the group's event.
   cudaStream_t s = c->stream, sp = c->prep_stream;
@@ -911,7 +954,7 @@ int lm_tri_run(lm_ctx *c) {
     a.fast = lm::tri_fast(p);
     if ((rc = initial_cap(*c, plan, a.fast, a.cap))) return rc;
     a.group_has_kernel.assign(plan.n_groups, 0);
-    // groups of whole source images: sort + node kernel of group g overlap the upload of group g+1
+    // groups of whole source images: row placement + node kernel of group g overlap the upload of group g+1
     for (int g = 0, b0 = 0, v0 = plan.vb; g < plan.n_groups; ++g) {
       const int b1 = group_end(plan, g, b0), v1 = (b1 < plan.nb) ? plan.blk[b1].src_view : plan.ve;
       if ((rc = queue_group(c, plan, p, g, b0, b1, v0, v1, a))) return rc;

@@ -117,8 +117,8 @@ struct lm_ctx {
   // match uploads run on their own stream so that a run can start on the first source images while the rest
   // of the tables is still crossing PCIe
   cudaStream_t copy_stream = nullptr;
-  cudaStream_t prep_stream = nullptr; // row expansion + sort of pipeline group g+1 run under the node kernel of group g
-  std::vector<cudaEvent_t> evp;       // per pipeline group: rows of the group sorted, node offsets known
+  cudaStream_t prep_stream = nullptr; // node order of the rows of pipeline group g+1, under the node kernel of group g
+  std::vector<cudaEvent_t> evp;       // per pipeline group: rows of the group in node order, node offsets known
   cudaEvent_t ev_run_begin = nullptr;
   cudaStream_t out_stream = nullptr;  // device -> host copies of finished groups (lm_tri_set_node_sink)
   char *node_sink = nullptr;
@@ -175,14 +175,14 @@ struct lm_ctx {
   unsigned int *h_pin = nullptr;
   // run buffers
   DevBuf d_blk_row_off, d_blk_src, d_blk_ng, d_blk_pair_off;
-  DevBuf d_key, d_key2, d_val, d_val2, d_sort_tmp;
+  DevBuf d_row_ng, d_sort_tmp; // match rows in node order: (ng_view << 16) | ng_line
+  // row chunks of the blocks and the shard's per-view tables; per (line, row chunk): row count and first row
+  DevBuf d_blk_chunks, d_blk_chunk_off, d_view_chunk_off, d_view_ent, d_view_tab_off, d_view_row_off, d_row_cnt, d_row_pos;
   DevBuf d_node_row_off, d_scalars; // scalars: [0] max_rows(uint) [1] err(int) ; counters at +16
   DevBuf d_nodes, d_row_state, d_row_cand, d_slab;
   DevBuf d_edges, d_edges2, d_edge_keys, d_edge_keys2, d_edge_w, d_edge_cnt;
   DevBuf d_g_flag, d_g_pos, d_g_kc, d_g_wc, d_g_occ, d_g_occ2, d_g_hk, d_g_hk2, d_g_gidx, d_g_gnode, d_g_k1, d_g_k1b, d_g_k2, d_g_k2b;
   DevBuf d_nvalid, d_edge_off, d_edge_ng; // compact valid_edges_ of the shard (node-major, candidate order)
-  uint32_t *sorted_val = nullptr;
-  uint32_t *sorted_key = nullptr;
   int64_t n_rows = 0;
   int64_t node_begin = 0, node_end = 0;
   bool ran = false;

@@ -87,15 +87,29 @@ void launch_group_edges(const uint8_t *row_state, const uint32_t *row_ng, const 
 void launch_scene_prepare(const double *segs_raw, int64_t n_nodes, double add, const int64_t *line_off, int n_views,
                           double *segs, uint16_t *node_view, cudaStream_t s);
 cudaError_t launch_tri_node_kernel(const TriParams &p, int grid, size_t smem, cudaStream_t s);
-void launch_expand_rows(const int32_t *d_pairs, const int64_t *d_blk_row_off, const int32_t *d_blk_src_view,
-                        const int32_t *d_blk_ng_view, const int64_t *d_blk_pair_off, int n_blocks,
-                        const int64_t *d_line_off, int64_t r_begin, int64_t r_end, uint32_t *d_key, uint32_t *d_val,
-                        int *d_err, cudaStream_t s);
-void launch_expand_exhaustive(const int64_t *d_blk_row_off, const int32_t *d_blk_src_view,
-                              const int32_t *d_blk_ng_view, int n_blocks, const int64_t *d_line_off,
-                              int64_t n_rows, uint32_t *d_key, uint32_t *d_val, cudaStream_t s);
-void launch_node_offsets(const uint32_t *d_sorted_key, int64_t n_rows, int64_t row_base, int64_t node_lo,
-                         int64_t node_hi, uint32_t *d_node_row_off, unsigned int *d_max_rows, cudaStream_t s);
+// Match rows -> node-major rows (tri_plumbing.cu). Every block of a run is cut into chunks of at most kRowChunk rows
+// (fewer than 2^16: a chunk's line counts are 16-bit). The shard's block and view tables, all on the device:
+struct RowTables {
+  const int64_t *blk_row_off;    // [nb+1] first flat row of every block
+  const int32_t *blk_src, *blk_ng; // [nb] source and neighbour view of every block
+  const int64_t *blk_pair_off;   // [nb] first pair of every block in the match store
+  const int32_t *blk_chunk_off;  // [nb+1] first chunk of every block
+  int nb;
+  const int64_t *line_off;       // [V+1] first node of every view
+  const int32_t *view_chunk_off; // [V+1] first chunk of every view of the shard
+  const int32_t *view_tab_off;   // [V+1] first count-table entry of every view of the shard (lines x chunks)
+  const int64_t *view_row_off;   // [V+1] first flat row of every view of the shard
+};
+constexpr int kRowChunk = 8192;
+void launch_view_tables(const RowTables &t, int vb, int ve, int32_t *view_ent, cudaStream_t s);
+cudaError_t launch_row_count(const RowTables &t, const int32_t *pairs, int k0, int n_chunks, int nl_max, uint16_t *cnt,
+                             int *err, cudaStream_t s);
+cudaError_t launch_row_place(const RowTables &t, const int32_t *pairs, int k0, int n_chunks, int nl_max,
+                             const uint32_t *pos, int64_t row_base, uint32_t *row_ng, cudaStream_t s);
+void launch_place_exhaustive(const RowTables &t, int64_t n_rows, uint32_t *row_ng, cudaStream_t s);
+void launch_node_row_off(const RowTables &t, const uint32_t *pos, int64_t t_end, int64_t row_base, int64_t row_end,
+                         int64_t node_lo, int64_t node_hi, int n_views, int exhaustive, uint32_t *off,
+                         unsigned int *max_rows, cudaStream_t s);
 void launch_extract_nvalid(const NodeRecord *nodes, int64_t node_begin, int64_t n, uint32_t *out, cudaStream_t s);
 void launch_edge_pairs(const uint32_t *edge_off, const uint32_t *edge_ng, const int64_t *line_off,
                        int64_t node_begin, int64_t n_nodes, int64_t n_edges, int64_t *out, cudaStream_t s);
@@ -113,7 +127,7 @@ struct RawBlock {
 void launch_block_keys(const RawBlock *raw, int n_all, int vb, int ve, int exhaustive, uint32_t *key, uint32_t *val,
                        cudaStream_t s);
 void launch_block_gather(const RawBlock *raw, const uint32_t *sorted_idx, int nb, int32_t *blk_src, int32_t *blk_ng,
-                         int64_t *blk_pair_off, int64_t *blk_rows, cudaStream_t s);
+                         int64_t *blk_pair_off, int64_t *blk_rows, int32_t *blk_chunks, cudaStream_t s);
 void launch_edge_weights(const EdgeParams &p, cudaStream_t s);
 void launch_gather_pack(const NodeRecord *nodes, int64_t node_begin, int64_t n_nodes, int64_t max_nodes,
                         const uint32_t *edge_off, const uint32_t *edge_ng, const int64_t *line_off, int64_t cap_edges,

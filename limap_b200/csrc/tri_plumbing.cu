@@ -1,7 +1,8 @@
 // tri_plumbing.cu — the plumbing kernels of the line-triangulation path (DESIGN.md §3.3): block tables, match rows ->
 // node-major rows and node offsets, valid-connection compaction and the host edge export, scene preparation, the
 // multi-GPU pack / unpack and run_clustering's edge weights.
-//   expand_rows / node_offsets : turn the per-(image, neighbour) match tables into node-major rows.
+//   view_tables / row_count / row_place / node_row_off : turn the per-(image, neighbour) match tables into node-major
+//       rows and every node's row range.
 //   group_edges / edge_pairs / edge_weights : run_clustering's edge list and 3d scores
 //       (global_line_triangulator.cc:234-291).
 #include "tri_kernels.cuh"
@@ -24,15 +25,17 @@ __global__ void block_keys_kernel(const RawBlock *__restrict__ raw, int n_all, i
 }
 __global__ void block_gather_kernel(const RawBlock *__restrict__ raw, const uint32_t *__restrict__ sorted_idx, int nb,
                                     int32_t *__restrict__ blk_src, int32_t *__restrict__ blk_ng,
-                                    int64_t *__restrict__ blk_pair_off, int64_t *__restrict__ blk_rows) {
+                                    int64_t *__restrict__ blk_pair_off, int64_t *__restrict__ blk_rows,
+                                    int32_t *__restrict__ blk_chunks) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i > nb) return;
-  if (i == nb) { blk_rows[i] = 0; return; }
+  if (i == nb) { blk_rows[i] = 0; blk_chunks[i] = 0; return; }
   const RawBlock b = raw[sorted_idx[i]];
   blk_src[i] = b.src_view;
   blk_ng[i] = b.ng_view;
   blk_pair_off[i] = b.pair_off;
   blk_rows[i] = b.n_rows;
+  blk_chunks[i] = (int32_t)((b.n_rows + kRowChunk - 1) / kRowChunk);
 }
 void launch_block_keys(const RawBlock *raw, int n_all, int vb, int ve, int exhaustive, uint32_t *key, uint32_t *val,
                        cudaStream_t s) {
@@ -40,8 +43,9 @@ void launch_block_keys(const RawBlock *raw, int n_all, int vb, int ve, int exhau
   block_keys_kernel<<<(n_all + 255) / 256, 256, 0, s>>>(raw, n_all, vb, ve, exhaustive, key, val);
 }
 void launch_block_gather(const RawBlock *raw, const uint32_t *sorted_idx, int nb, int32_t *blk_src, int32_t *blk_ng,
-                         int64_t *blk_pair_off, int64_t *blk_rows, cudaStream_t s) {
-  block_gather_kernel<<<(nb + 1 + 255) / 256, 256, 0, s>>>(raw, sorted_idx, nb, blk_src, blk_ng, blk_pair_off, blk_rows);
+                         int64_t *blk_pair_off, int64_t *blk_rows, int32_t *blk_chunks, cudaStream_t s) {
+  block_gather_kernel<<<(nb + 1 + 255) / 256, 256, 0, s>>>(raw, sorted_idx, nb, blk_src, blk_ng, blk_pair_off, blk_rows,
+                                                           blk_chunks);
 }
 __global__ void zero_words_kernel(unsigned int *p, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -53,92 +57,208 @@ void launch_zero_words(void *d_dst, int n_words, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Match tables -> node-major rows. Flat row order = (source view asc, neighbour view asc, row), the
-// order in which TriangulateImage appends to tris_ (base_line_triangulator.cc:74-100); a stable sort
-// by node id then yields each node's candidates in reference order.
-__global__ void expand_rows_kernel(const int32_t *__restrict__ pairs, const int64_t *__restrict__ blk_row_off,
-                                   const int32_t *__restrict__ blk_src, const int32_t *__restrict__ blk_ng,
-                                   const int64_t *__restrict__ blk_pair_off, int n_blocks,
-                                   const int64_t *__restrict__ line_off, int64_t r_begin, int64_t n_rows,
-                                   uint32_t *__restrict__ key, uint32_t *__restrict__ val, int *err) {
-  for (int64_t r = r_begin + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_rows;
-       r += (int64_t)gridDim.x * blockDim.x) {
-    const int b = last_le(blk_row_off, n_blocks, r);
-    const int64_t q = blk_pair_off[b] + (r - blk_row_off[b]);
-    const int2 pr = reinterpret_cast<const int2 *>(pairs)[q];
-    const int sv = blk_src[b], nv = blk_ng[b];
-    const int64_t nl_src = line_off[sv + 1] - line_off[sv];
-    const int64_t nl_ng = line_off[nv + 1] - line_off[nv];
-    int line = pr.x, ngl = pr.y;
-    if (line < 0 || line >= nl_src) { *err = 1; line = 0; }
-    if (ngl < 0 || ngl >= nl_ng) { *err = 2; ngl = 0; }
-    key[r] = (uint32_t)(line_off[sv] + line);
-    val[r] = ((uint32_t)nv << 16) | (uint32_t)ngl;
+// Match tables -> node-major rows. Flat row order = (source view asc, neighbour view asc, row), the order in which
+// TriangulateImage appends to tris_ (base_line_triangulator.cc:74-100). The rows of one source view already occupy the
+// output range they end up in, so putting them in node order is a stable bucketing by line inside that range, and every
+// node gets its candidates in (block, row) order, the reference's order.
+//
+// Every block is cut into chunks of at most kRowChunk rows (a chunk never spans blocks, so no kernel searches the block
+// of a row). row_count counts the rows of every line of the source view per chunk into a table laid out per source view
+// as [line][chunk of the view]. One exclusive scan over a pipeline group's slice of that table gives the first row of
+// every (line, chunk) relative to the group's first row; the entry of a line's first chunk is its node's first row.
+// row_place then writes each chunk's rows there, in order. Only one CTA advances a chunk's positions: no atomics, and
+// the result is deterministic.
+
+// lower_bound(blk_src[0, nb), v): the first block whose source view is v or later
+LM_D int first_block_of(const int32_t *__restrict__ blk_src, int nb, int v) {
+  int lo = 0, hi = nb;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (blk_src[mid] < v) lo = mid + 1; else hi = mid;
   }
+  return lo;
 }
-void launch_expand_rows(const int32_t *d_pairs, const int64_t *d_blk_row_off, const int32_t *d_blk_src_view,
-                        const int32_t *d_blk_ng_view, const int64_t *d_blk_pair_off, int n_blocks,
-                        const int64_t *d_line_off, int64_t r_begin, int64_t r_end, uint32_t *d_key, uint32_t *d_val,
-                        int *d_err, cudaStream_t s) {
-  if (r_end <= r_begin) return;
-  int grid = (int)((r_end - r_begin + 255) / 256);
-  grid = std::min(grid, current_device_sms() * 16);
-  expand_rows_kernel<<<grid, 256, 0, s>>>(d_pairs, d_blk_row_off, d_blk_src_view, d_blk_ng_view, d_blk_pair_off,
-                                          n_blocks, d_line_off, r_begin, r_end, d_key, d_val, d_err);
+// The per-view tables of the shard's views [vb, ve]: first chunk, first flat row and count-table entries (lines x chunks).
+__global__ void view_tables_kernel(const int32_t *__restrict__ blk_src, const int32_t *__restrict__ blk_chunk_off,
+                                   const int64_t *__restrict__ blk_row_off, int nb, const int64_t *__restrict__ line_off,
+                                   int vb, int ve, int32_t *__restrict__ view_chunk_off,
+                                   int64_t *__restrict__ view_row_off, int32_t *__restrict__ view_ent) {
+  const int v = vb + blockIdx.x * blockDim.x + threadIdx.x;
+  if (v > ve) return;
+  const int b = first_block_of(blk_src, nb, v);
+  view_chunk_off[v] = blk_chunk_off[b];
+  view_row_off[v] = blk_row_off[b];
+  view_ent[v] = 0;
+  if (v < ve)
+    view_ent[v] = (int32_t)((line_off[v + 1] - line_off[v]) * (blk_chunk_off[first_block_of(blk_src, nb, v + 1)] - blk_chunk_off[b]));
+}
+void launch_view_tables(const RowTables &t, int vb, int ve, int32_t *view_ent, cudaStream_t s) {
+  view_tables_kernel<<<(ve - vb + 1 + 255) / 256, 256, 0, s>>>(t.blk_src, t.blk_chunk_off, t.blk_row_off, t.nb, t.line_off,
+                                                               vb, ve, const_cast<int32_t *>(t.view_chunk_off),
+                                                               const_cast<int64_t *>(t.view_row_off), view_ent);
 }
 
-// TriangulateImageExhaustiveMatch (base_line_triangulator.cc:111-136): every line of the neighbour.
-__global__ void expand_exhaustive_kernel(const int64_t *__restrict__ blk_row_off, const int32_t *__restrict__ blk_src,
-                                         const int32_t *__restrict__ blk_ng, int n_blocks,
-                                         const int64_t *__restrict__ line_off, int64_t n_rows,
-                                         uint32_t *__restrict__ key, uint32_t *__restrict__ val) {
-  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
-    const int b = last_le(blk_row_off, n_blocks, r);
-    const int64_t q = r - blk_row_off[b];
-    const int sv = blk_src[b], nv = blk_ng[b];
-    const int64_t nl_ng = line_off[nv + 1] - line_off[nv];
-    key[r] = (uint32_t)(line_off[sv] + q / nl_ng);
-    val[r] = ((uint32_t)nv << 16) | (uint32_t)(q % nl_ng);
+// Chunk k of the shard: its rows [r0, r1) and first match pair, its views and line counts, its column of the count table.
+struct RowChunk {
+  int64_t r0, r1, q0, tab; // tab: entry of line 0; line l at tab + l * nch
+  int sv, nv, nl, nl_ng, nch;
+};
+LM_D RowChunk row_chunk(const RowTables &t, int k) {
+  RowChunk c;
+  const int b = last_le(t.blk_chunk_off, t.nb, k);
+  const int64_t j = (int64_t)(k - t.blk_chunk_off[b]) * kRowChunk;
+  c.r0 = t.blk_row_off[b] + j;
+  c.r1 = min(c.r0 + kRowChunk, t.blk_row_off[b + 1]);
+  c.q0 = t.blk_pair_off[b] + j;
+  c.sv = t.blk_src[b];
+  c.nv = t.blk_ng[b];
+  c.nl = (int)(t.line_off[c.sv + 1] - t.line_off[c.sv]);
+  c.nl_ng = (int)(t.line_off[c.nv + 1] - t.line_off[c.nv]);
+  c.nch = t.view_chunk_off[c.sv + 1] - t.view_chunk_off[c.sv];
+  c.tab = t.view_tab_off[c.sv] + (k - t.view_chunk_off[c.sv]);
+  return c;
+}
+
+constexpr int kRowThreads = 256;
+
+// Pass 1: rows per line of chunk k0 + blockIdx.x, and the IndexError flags (d_scalars word 1).
+__global__ void __launch_bounds__(kRowThreads) row_count_kernel(const __grid_constant__ RowTables t,
+                                                                const int32_t *__restrict__ pairs, int k0,
+                                                                uint16_t *__restrict__ cnt, int *err) {
+  extern __shared__ uint32_t lc[]; // two 16-bit line counters per word (a chunk has fewer than 2^16 rows)
+  const RowChunk c = row_chunk(t, k0 + blockIdx.x);
+  for (int i = threadIdx.x; i < (c.nl + 1) / 2; i += kRowThreads) lc[i] = 0u;
+  __syncthreads();
+  const int2 *pr = reinterpret_cast<const int2 *>(pairs) + c.q0;
+  const int n = (int)(c.r1 - c.r0);
+  for (int i = threadIdx.x; i < n; i += kRowThreads) {
+    const int2 m = pr[i];
+    int line = m.x;
+    if (line < 0 || line >= c.nl) { *err = 1; line = 0; }
+    if (m.y < 0 || m.y >= c.nl_ng) *err = 2;
+    if (c.nl > 0) atomicAdd(&lc[line >> 1], 1u << ((line & 1) * 16));
+  }
+  __syncthreads();
+  for (int l = threadIdx.x; l < c.nl; l += kRowThreads)
+    cnt[c.tab + (int64_t)l * c.nch] = (uint16_t)(lc[l >> 1] >> ((l & 1) * 16));
+}
+
+// Pass 2: the rows of chunk k0 + blockIdx.x at their node-major positions (pos: the scanned count table, relative to
+// row_base). A tile of kRowThreads rows at a time: a row's rank among the equal lines of its warp comes from
+// __match_any_sync, and the warps take turns, in row order, to advance the chunk's running count of each line.
+__global__ void __launch_bounds__(kRowThreads) row_place_kernel(const __grid_constant__ RowTables t,
+                                                                const int32_t *__restrict__ pairs, int k0,
+                                                                const uint32_t *__restrict__ pos, int64_t row_base,
+                                                                uint32_t *__restrict__ row_ng) {
+  extern __shared__ uint16_t run[]; // rows of every line this chunk has placed so far
+  const RowChunk c = row_chunk(t, k0 + blockIdx.x);
+  for (int l = threadIdx.x; l < c.nl; l += kRowThreads) run[l] = 0;
+  __syncthreads();
+  if (c.nl == 0) return; // (every row is out of range: row_count raised the IndexError)
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int2 *pr = reinterpret_cast<const int2 *>(pairs) + c.q0;
+  const int n = (int)(c.r1 - c.r0);
+  int2 next = threadIdx.x < n ? pr[threadIdx.x] : make_int2(0, 0);
+  for (int i0 = 0; i0 < n; i0 += kRowThreads) {
+    const int i = i0 + threadIdx.x;
+    const bool valid = i < n;
+    const int2 m = next;
+    if (i + kRowThreads < n) next = pr[i + kRowThreads];
+    int line = m.x, ngl = m.y;
+    if (line < 0 || line >= c.nl) line = 0;
+    if (ngl < 0 || ngl >= c.nl_ng) ngl = 0;
+    const unsigned same = __match_any_sync(0xffffffffu, valid ? line : -1);
+    const unsigned before = same & ((1u << lane) - 1u);
+    const bool head = valid && before == 0u; // the first row of its line in this warp
+    uint32_t base = head ? __ldg(&pos[c.tab + (int64_t)line * c.nch]) : 0u;
+    for (int w = 0; w < kRowThreads / 32; ++w) {
+      if (w == warp && head) {
+        const uint16_t k = run[line];
+        run[line] = (uint16_t)(k + __popc(same));
+        base += k;
+      }
+      __syncthreads();
+    }
+    base = __shfl_sync(0xffffffffu, base, __ffs(same) - 1);
+    if (valid) row_ng[row_base + base + __popc(before)] = ((uint32_t)c.nv << 16) | (uint32_t)ngl;
   }
 }
-void launch_expand_exhaustive(const int64_t *d_blk_row_off, const int32_t *d_blk_src_view,
-                              const int32_t *d_blk_ng_view, int n_blocks, const int64_t *d_line_off, int64_t n_rows,
-                              uint32_t *d_key, uint32_t *d_val, cudaStream_t s) {
-  if (n_rows == 0) return;
+
+static cudaError_t set_smem(const void *f, size_t smem) {
+  return smem > 48 * 1024 ? cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                          : cudaSuccess;
+}
+cudaError_t launch_row_count(const RowTables &t, const int32_t *pairs, int k0, int n_chunks, int nl_max, uint16_t *cnt,
+                             int *err, cudaStream_t s) {
+  if (n_chunks <= 0) return cudaSuccess;
+  const size_t smem = 4 * (size_t)((nl_max + 1) / 2);
+  cudaError_t e = set_smem((const void *)row_count_kernel, smem);
+  if (e != cudaSuccess) return e;
+  row_count_kernel<<<n_chunks, kRowThreads, smem, s>>>(t, pairs, k0, cnt, err);
+  return cudaGetLastError();
+}
+cudaError_t launch_row_place(const RowTables &t, const int32_t *pairs, int k0, int n_chunks, int nl_max,
+                             const uint32_t *pos, int64_t row_base, uint32_t *row_ng, cudaStream_t s) {
+  if (n_chunks <= 0) return cudaSuccess;
+  const size_t smem = 4 * (size_t)((nl_max + 1) / 2);
+  cudaError_t e = set_smem((const void *)row_place_kernel, smem);
+  if (e != cudaSuccess) return e;
+  row_place_kernel<<<n_chunks, kRowThreads, smem, s>>>(t, pairs, k0, pos, row_base, row_ng);
+  return cudaGetLastError();
+}
+
+// TriangulateImageExhaustiveMatch (base_line_triangulator.cc:111-136): every line of the source view gets every line of
+// every neighbour, so a row's position is closed-form: its node's first row plus the lines of the earlier neighbours.
+__global__ void place_exhaustive_kernel(const __grid_constant__ RowTables t, int64_t n_rows, uint32_t *__restrict__ row_ng) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
+    const int b = last_le(t.blk_row_off, t.nb, r);
+    const int sv = t.blk_src[b], nv = t.blk_ng[b];
+    const int64_t nl = t.line_off[sv + 1] - t.line_off[sv], nl_ng = t.line_off[nv + 1] - t.line_off[nv];
+    const int64_t q = r - t.blk_row_off[b], v0 = t.view_row_off[sv];
+    const int64_t per_line = (t.view_row_off[sv + 1] - v0) / nl;
+    row_ng[v0 + (q / nl_ng) * per_line + (t.blk_row_off[b] - v0) / nl + q % nl_ng] =
+        ((uint32_t)nv << 16) | (uint32_t)(q % nl_ng);
+  }
+}
+void launch_place_exhaustive(const RowTables &t, int64_t n_rows, uint32_t *row_ng, cudaStream_t s) {
+  if (n_rows <= 0) return;
   int grid = (int)((n_rows + 255) / 256);
   grid = std::min(grid, current_device_sms() * 16);
-  expand_exhaustive_kernel<<<grid, 256, 0, s>>>(d_blk_row_off, d_blk_src_view, d_blk_ng_view, n_blocks, d_line_off,
-                                                n_rows, d_key, d_val);
+  place_exhaustive_kernel<<<grid, 256, 0, s>>>(t, n_rows, row_ng);
 }
 
-// Row range of every node in [node_lo, node_hi] from the node-sorted keys of one group (rows
-// [row_base, row_base + n_rows) of the run); off[n] is a row index of the whole run.
-__global__ void node_offsets_kernel(const uint32_t *__restrict__ key, int64_t n_rows, int64_t row_base,
-                                    int64_t node_lo, int64_t node_hi, uint32_t *__restrict__ off,
-                                    unsigned int *max_rows) {
+// Row range of every node in [node_lo, node_hi] of one pipeline group, whose rows are [row_base, row_end) of the run;
+// off[n] is a row index of the whole run and off[node_hi] = row_end. Matches: from the group's scanned count table,
+// entries [.., t_end). Exhaustive matching: every line of a source view has the same number of rows. The largest node
+// goes to max_rows.
+__global__ void node_row_off_kernel(const __grid_constant__ RowTables t, const uint32_t *__restrict__ pos, int64_t t_end,
+                                    int64_t row_base, int64_t row_end, int64_t node_lo, int64_t node_hi, int n_views,
+                                    int exhaustive, uint32_t *__restrict__ off, unsigned int *max_rows) {
   const int64_t n = node_lo + blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (n > node_hi) return;
-  int64_t lo = 0, hi = n_rows; // lower_bound(key, n)
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if (key[mid] < (uint32_t)n) lo = mid + 1; else hi = mid;
+  if (n == node_hi) { off[n] = (uint32_t)row_end; return; }
+  const int sv = last_le(t.line_off, n_views, n);
+  const int64_t l = n - t.line_off[sv];
+  int64_t first, cnt;
+  if (exhaustive) {
+    cnt = (t.view_row_off[sv + 1] - t.view_row_off[sv]) / (t.line_off[sv + 1] - t.line_off[sv]);
+    first = t.view_row_off[sv] + l * cnt;
+  } else {
+    const int64_t nch = t.view_chunk_off[sv + 1] - t.view_chunk_off[sv];
+    const int64_t i = t.view_tab_off[sv] + l * nch, tot = row_end - row_base;
+    const int64_t a = i < t_end ? (int64_t)pos[i] : tot, b = i + nch < t_end ? (int64_t)pos[i + nch] : tot;
+    first = row_base + a;
+    cnt = b - a;
   }
-  off[n] = (uint32_t)(row_base + lo);
-  if (n < node_hi) {
-    int64_t lo2 = lo, hi2 = n_rows;
-    while (lo2 < hi2) {
-      const int64_t mid = (lo2 + hi2) >> 1;
-      if (key[mid] < (uint32_t)(n + 1)) lo2 = mid + 1; else hi2 = mid;
-    }
-    const unsigned int cnt = (unsigned int)(lo2 - lo);
-    if (cnt) atomicMax(max_rows, cnt);
-  }
+  off[n] = (uint32_t)first;
+  if (cnt) atomicMax(max_rows, (unsigned int)cnt);
 }
-void launch_node_offsets(const uint32_t *d_sorted_key, int64_t n_rows, int64_t row_base, int64_t node_lo,
-                         int64_t node_hi, uint32_t *d_node_row_off, unsigned int *d_max_rows, cudaStream_t s) {
+void launch_node_row_off(const RowTables &t, const uint32_t *pos, int64_t t_end, int64_t row_base, int64_t row_end,
+                         int64_t node_lo, int64_t node_hi, int n_views, int exhaustive, uint32_t *off,
+                         unsigned int *max_rows, cudaStream_t s) {
   const int grid = (int)((node_hi - node_lo + 1 + 255) / 256);
-  node_offsets_kernel<<<grid, 256, 0, s>>>(d_sorted_key, n_rows, row_base, node_lo, node_hi, d_node_row_off,
-                                           d_max_rows);
+  node_row_off_kernel<<<grid, 256, 0, s>>>(t, pos, t_end, row_base, row_end, node_lo, node_hi, n_views, exhaustive, off,
+                                           max_rows);
 }
 
 // valid_edges_ (global_line_triangulator.cc:130-142) in compact, node-major, candidate-ordered form.
