@@ -449,6 +449,49 @@ int lm_loc_solve(lm_ctx *ctx, int64_t n_queries, const double *kvec, const doubl
 /* Sizes, iteration totals and times of the last lm_loc_solve. */
 int lm_loc_get_stats(lm_ctx *ctx, lm_loc_stats *out);
 
+/* ---- line matching of query images against a line map (localization) --------------------------------------------
+ * Replaces the Python double loops of optimize/hybrid_localization/functions.py as runners/hybrid_localization.py calls
+ * them, for every query and every retrieved database image in one pass. An item is a (query image, target image) pair;
+ * items come in query order, then retrieval order, and a query is a run of items with the same query image. Every
+ * output list keeps the reference's order. Outputs stay on the device until lm_locmatch_get: a caller sizes its buffers
+ * from the returned count, then fetches. */
+typedef struct lm_locmatch_stats {
+  int64_t n_items, n_tests;  /* items and IoU tests of the last sweep or filter */
+  int64_t n_pairs_2to2;      /* pairs past the IoU test (tracked or not) */
+  int64_t n_out;             /* pairs in the last result */
+  double kernel_ms;          /* device time of the last call's kernels, host waits between them excluded */
+  double test_ms;            /* device time of the IoU test kernel of the last sweep or filter */
+  double total_ms;           /* host wall time of the last call, copies included */
+} lm_locmatch_stats;
+
+/* The scene: n_images images with kvec[n][4] = fx, fy, cx, cy, qvec[n][4] (w, x, y, z), tvec[n][3]; their 2D lines as
+ * line_off[n+1] into lines[][4]; line_track[] the track of every line (-1: untracked; the inverse id map of
+ * base.get_invert_idmap_from_linetracks, base/functions.py:50-72; NULL without a map) and the tracks' lines
+ * track_lines[n_tracks][6] (start, end). */
+int lm_locmatch_set_scene(lm_ctx *ctx, int32_t n_images, const double *kvec, const double *qvec, const double *tvec,
+                          const int64_t *line_off, const double *lines, const int32_t *line_track, int64_t n_tracks,
+                          const double *track_lines);
+/* match_line_2to2_epipolarIoU (functions.py:6-23) of every item items[n][2] = (query image, target image): the pairs
+ * (query line, target line) with compute_epipolar_IoU > IoU_threshold, query line major. to_tracks: fused with
+ * match_line_2to3 (functions.py:55-66), pairs (query line, track) of the tracked target lines only. Returns the number
+ * of pairs; lm_locmatch_get gives them with offsets per item. */
+int64_t lm_locmatch_sweep(lm_ctx *ctx, int64_t n_items, const int32_t *items, double IoU_threshold, int32_t to_tracks);
+/* filter_line_2to2_epipolarIoU (functions.py:26-52) of given pairs: pair_off[n_items+1] into pairs[][2] = (query line,
+ * target line) per item, kept in order when compute_epipolar_IoU > IoU_threshold (every pair when use_iou is 0).
+ * to_tracks as for lm_locmatch_sweep. Returns the number of pairs kept. */
+int64_t lm_locmatch_filter(lm_ctx *ctx, int64_t n_items, const int32_t *items, const int64_t *pair_off,
+                           const int32_t *pairs, int32_t use_iou, double IoU_threshold, int32_t to_tracks);
+/* The (query line, track) pairs of the last to_tracks sweep or filter, grouped per query as the runner's defaultdict
+ * all_line_pairs_2to3 holds them (runners/hybrid_localization.py:284-346): query lines in order of first appearance,
+ * tracks in append order, duplicates kept. dist_func -1 returns that list; 0 perpendicular_dist, 1 midpoint_dist,
+ * 2 midpoint_perpendicular_dist apply reprojection_filter_matches_2to3 (functions.py:96-140) with the query image's
+ * camera and dist_thres, sine_thres, angle_scale, one pair per query line at most. Returns the number of pairs;
+ * lm_locmatch_get gives them with offsets per query. */
+int64_t lm_locmatch_group(lm_ctx *ctx, int32_t dist_func, double dist_thres, double sine_thres, double angle_scale);
+/* The last result: off[n+1] (n items for sweep / filter, n queries for group) and pairs[cap][2]; cap must hold them. */
+int lm_locmatch_get(lm_ctx *ctx, int64_t *off, int32_t *pairs, int64_t cap);
+int lm_locmatch_get_stats(lm_ctx *ctx, lm_locmatch_stats *out);
+
 #ifdef __cplusplus
 }
 #endif

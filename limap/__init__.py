@@ -17,3 +17,6 @@ for _name in ("base", "triangulation", "optimize", "vplib", "merging", "util", "
 if "limap.optimize" in sys.modules:
     sys.modules["limap.optimize.hybrid_localization"] = sys.modules["limap_b200.hybrid_localization"]
     sys.modules["limap.optimize.hybrid_localization.solve"] = sys.modules["limap_b200.hybrid_localization"]
+    _fn = importlib.import_module("limap_b200.hybrid_localization_functions")
+    sys.modules["limap.optimize.hybrid_localization.functions"] = _fn
+    sys.modules["limap_b200.hybrid_localization"].functions = _fn

@@ -77,6 +77,11 @@ class LocStats(C.Structure):
                 ("total_successful", C.c_int64), ("kernel_ms", C.c_double), ("total_ms", C.c_double)]
 
 
+class LocMatchStats(C.Structure):
+    _fields_ = [("n_items", C.c_int64), ("n_tests", C.c_int64), ("n_pairs_2to2", C.c_int64), ("n_out", C.c_int64),
+                ("kernel_ms", C.c_double), ("test_ms", C.c_double), ("total_ms", C.c_double)]
+
+
 NODE_RECORD_DTYPE = np.dtype([("line", np.float64, 9), ("score", np.float64), ("ng_view", np.int32),
                               ("ng_line", np.int32), ("n_cand", np.int32), ("n_valid", np.int32)])
 
@@ -148,6 +153,12 @@ _SIGS = {
     "lm_eval_mesh_line_inliers": (C.c_int, [_P, C.c_int64, _P, C.c_int32, C.c_int32, _P, _P, _P]),
     "lm_loc_solve": (C.c_int, [_P, C.c_int64] + [_P] * 16),
     "lm_loc_get_stats": (C.c_int, [_P, _P]),
+    "lm_locmatch_set_scene": (C.c_int, [_P, C.c_int32] + [_P] * 6 + [C.c_int64, _P]),
+    "lm_locmatch_sweep": (C.c_int64, [_P, C.c_int64, _P, C.c_double, C.c_int32]),
+    "lm_locmatch_filter": (C.c_int64, [_P, C.c_int64, _P, _P, _P, C.c_int32, C.c_double, C.c_int32]),
+    "lm_locmatch_group": (C.c_int64, [_P, C.c_int32, C.c_double, C.c_double, C.c_double]),
+    "lm_locmatch_get": (C.c_int, [_P, _P, _P, C.c_int64]),
+    "lm_locmatch_get_stats": (C.c_int, [_P, _P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS)
 

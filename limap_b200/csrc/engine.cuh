@@ -237,6 +237,23 @@ struct lm_ctx {
   // query pose refinement (engine_loc.cu)
   DevBuf d_loc_in, d_loc_blocks, d_loc_out;
   lm_loc_stats loc_stats = {};
+  // localization line matching (engine_locmatch.cu): the scene, the last sweep / filter result E with its items, and
+  // the last result handed to lm_locmatch_get
+  struct LocMatch {
+    DevBuf views, line_off, lines, track, tracks;
+    int32_t n_images = 0;
+    int64_t n_lines = 0, n_tracks = 0;
+    bool has_map = false;
+    std::vector<int64_t> h_line_off;
+    DevBuf items, row_off, word_off, mask, cnt, scan, pair_off, pairs, flag, item_off, E, err;
+    DevBuf g_cnt, g_first, g_key, g_run, g_head, g_qhead, g_qtot, g_qoff, g_qrow, g_qout, G, pos, sel, out, small, tmp;
+    std::vector<int32_t> h_items;
+    std::vector<int64_t> h_item_off, h_out_off;
+    int64_t n_items = 0, n_e = 0, n_out = 0;
+    bool e_tracks = false;
+    int2 *d_out = nullptr;
+  } lmm;
+  lm_locmatch_stats lmm_stats = {};
   ~lm_ctx();
 };
 

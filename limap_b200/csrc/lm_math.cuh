@@ -118,6 +118,67 @@ template <typename T> LM_HD vec3<T> solve3_cols(vec3<T> a, vec3<T> b, vec3<T> c,
                 i20 * r.x + i21 * r.y + i22 * r.z);
 }
 
+// compute_epipolar_IoU (triangulation/functions.cc:76-98) of a source line in the segment l2 = (x1, y1, x2, y2) of a
+// second view. The epipolar lines of the source endpoints come from ep: ep.start() / ep.end() = F x1 up to scale. A value
+// within 1e-7 of th is recomputed in the reference's normalised form, so that the caller's own comparison with th decides
+// as the reference's does. A zero-length l2 gives NaN, as in the reference. s2, e2: the endpoints of l2, v2d = e2 - s2,
+// len2sq = |v2d|^2. dehomogeneous() of the cross product of two normalised line vectors == raw.xy / (raw.z + EPS |a| |b|).
+template <typename EP>
+LM_D double epipolar_iou(const EP &ep, double4 l2, vec2<double> s2, vec2<double> e2, vec2<double> v2d, double len2sq,
+                         const double &th) {
+  const vec3<double> l2h = cross(mk3(l2.x, l2.y, 1.0), mk3(l2.z, l2.w, 1.0));
+  const double nl2 = dot(l2h, l2h);
+  const vec3<double> eps_ = ep.start();
+  const vec3<double> hs = cross(l2h, eps_);
+  const double ws = 1.0 / (hs.z + consts<double>::eps() * sqrt(nl2 * dot(eps_, eps_)));
+  const vec3<double> epe_ = ep.end();
+  const vec3<double> he = cross(l2h, epe_);
+  const double we = 1.0 / (he.z + consts<double>::eps() * sqrt(nl2 * dot(epe_, epe_)));
+  const vec2<double> cs = mk2(hs.x * ws, hs.y * ws), ce = mk2(he.x * we, he.y * we);
+  const double il2 = 1.0 / len2sq;
+  double c1 = dot(cs - s2, v2d) * il2;
+  double c2 = dot(ce - s2, v2d) * il2;
+  if (c1 > c2) { double t = c1; c1 = c2; c2 = t; }
+  double IoU = (smin(c2, 1.0) - smax(c1, 0.0)) / (smax(c2, 1.0) - smin(c1, 0.0));
+  if (fabs(IoU - th) < 1e-7) {
+    // too close to the threshold: evaluate in the reference's normalised form
+    const vec3<double> coor_l2 = normalized(l2h);
+    const vec2<double> cs2 = dehom(cross(coor_l2, normalized(eps_)));
+    const vec2<double> ce2 = dehom(cross(coor_l2, normalized(epe_)));
+    const vec2<double> dir2 = normalized(v2d);
+    const double len2 = norm(s2 - e2);
+    c1 = dot(cs2 - s2, dir2) / len2;
+    c2 = dot(ce2 - s2, dir2) / len2;
+    if (c1 > c2) { double t = c1; c1 = c2; c2 = t; }
+    IoU = (smin(c2, 1.0) - smax(c1, 0.0)) / (smax(c2, 1.0) - smin(c1, 0.0));
+  }
+  return IoU;
+}
+template <typename EP> LM_D double epipolar_iou(const EP &ep, double4 l2, double th) {
+  const vec2<double> s2 = mk2(l2.x, l2.y), e2 = mk2(l2.z, l2.w);
+  const vec2<double> v2d = e2 - s2;
+  return epipolar_iou(ep, l2, s2, e2, v2d, dot(v2d, v2d), th);
+}
+// The epipolar lines from the source rays where they are used: F x1 = M2^T ((C1 - C2) x (M1 x1)) exactly
+// (F = K2^-T [t]x R2 R1^T K1^-1 with t = R2 (C1 - C2)). M2 = R2^T K2^-1 of the second view, base = C1 - C2, w1s / w1e =
+// M1 [p; 1] of the source endpoints, held by reference so that the node kernel loads them from shared memory where it
+// always did.
+struct EpipolarFromRays {
+  const double *M2;
+  vec3<double> base;
+  const vec3<double> &w1s, &w1e;
+  LM_D vec3<double> start() const { return mat3T_mul(M2, cross(base, w1s)); }
+  LM_D vec3<double> end() const { return mat3T_mul(M2, cross(base, w1e)); }
+};
+// The same lines computed once for every target line of a (source line, second view) pair.
+struct EpipolarLines {
+  vec3<double> s, e;
+  LM_D EpipolarLines(const double *M2, vec3<double> base, vec3<double> w1s, vec3<double> w1e)
+      : s(mat3T_mul(M2, cross(base, w1s))), e(mat3T_mul(M2, cross(base, w1e))) {}
+  LM_D vec3<double> start() const { return s; }
+  LM_D vec3<double> end() const { return e; }
+};
+
 // ------------------------------------------------------------------------------------------------
 // Segment helpers shared by the 2d and 3d linkers (base/line_dists.h).
 template <typename V> struct seg {

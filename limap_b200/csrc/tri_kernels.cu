@@ -235,39 +235,10 @@ LM_D bool cand_gates(const TriParams &p, const ViewD &v2, const Src &src, const 
     }
   }
   const vec3<double> C2 = mk3(v2.C[0], v2.C[1], v2.C[2]);
-  // compute_epipolar_IoU (functions.cc:76-98). F x1 = M2^T ((C1 - C2) x (M1 x1)) exactly
-  // (F = K2^-T [t]x R2 R1^T K1^-1 with t = R2 (C1 - C2)); dehomogeneous() of the cross product of two
-  // normalised line vectors == raw.xy / (raw.z + EPS |a| |b|).
-  {
-    const vec3<double> base = src.C1 - C2;
-    const vec3<double> l2h = cross(mk3(l2.x, l2.y, 1.0), mk3(l2.z, l2.w, 1.0));
-    const double nl2 = dot(l2h, l2h);
-    const vec3<double> eps_ = mat3T_mul(v2.M, cross(base, src.w1s));
-    const vec3<double> hs = cross(l2h, eps_);
-    const double ws = 1.0 / (hs.z + consts<double>::eps() * sqrt(nl2 * dot(eps_, eps_)));
-    const vec3<double> epe_ = mat3T_mul(v2.M, cross(base, src.w1e));
-    const vec3<double> he = cross(l2h, epe_);
-    const double we = 1.0 / (he.z + consts<double>::eps() * sqrt(nl2 * dot(epe_, epe_)));
-    const vec2<double> cs = mk2(hs.x * ws, hs.y * ws), ce = mk2(he.x * we, he.y * we);
-    const double il2 = 1.0 / len2sq;
-    double c1 = dot(cs - s2, v2d) * il2;
-    double c2 = dot(ce - s2, v2d) * il2;
-    if (c1 > c2) { double t = c1; c1 = c2; c2 = t; }
-    double IoU = (smin(c2, 1.0) - smax(c1, 0.0)) / (smax(c2, 1.0) - smin(c1, 0.0));
-    if (fabs(IoU - p.IoU_threshold) < 1e-7) {
-      // too close to the threshold: evaluate in the reference's normalised form
-      const vec3<double> coor_l2 = normalized(l2h);
-      const vec2<double> cs2 = dehom(cross(coor_l2, normalized(eps_)));
-      const vec2<double> ce2 = dehom(cross(coor_l2, normalized(epe_)));
-      const vec2<double> dir2 = normalized(v2d);
-      const double len2 = norm(s2 - e2);
-      c1 = dot(cs2 - s2, dir2) / len2;
-      c2 = dot(ce2 - s2, dir2) / len2;
-      if (c1 > c2) { double t = c1; c1 = c2; c2 = t; }
-      IoU = (smin(c2, 1.0) - smax(c1, 0.0)) / (smax(c2, 1.0) - smin(c1, 0.0));
-    }
-    if (IoU < p.IoU_threshold) return false;
-  }
+  // compute_epipolar_IoU (functions.cc:76-98); rejects on IoU < th, so NaN and IoU == th pass
+  if (epipolar_iou(EpipolarFromRays{v2.M, src.C1 - C2, src.w1s, src.w1e}, l2, s2, e2, v2d, len2sq, p.IoU_threshold) <
+      p.IoU_threshold)
+    return false;
   return true;
 }
 

@@ -1,15 +1,17 @@
-"""limap.runners as far as the triangulation path needs it: `setup`, the LOAD branches of `compute_2d_segs` /
+"""limap.runners as far as the triangulation and localization paths need it: `setup`, the LOAD branches of `compute_2d_segs` /
 `compute_matches` (detections and matches come from disk or from a GPU matcher; the learned front end is out of scope)
 and `line_triangulation` -- the steps of src/limap/runners/line_triangulation.py:18-245 ([A] metainfos, [B] segments,
 [C] matches, [D] triangulation + track filters + remerge, [E] line bundle adjustment, [F] output + track report) driven
-through this package's operator surface. tests/test_runner_dropin.py additionally executes the reference's own runner
+through this package's operator surface, and `hybrid_localization` (src/limap/runners/hybrid_localization.py:94-398) with
+the epipolar matcher or loaded learned matches and the ransac.method None estimator. tests/test_runner_dropin.py additionally executes the reference's own runner
 file, unmodified and loaded by path, against the same surface."""
 import logging
 import os
 
 import numpy as np
 
-from . import base, merging, optimize, triangulation, visualize, vplib
+from . import base, estimators, merging, optimize, triangulation, visualize, vplib
+from . import hybrid_localization_functions as _locfn
 from .util import io as limapio
 
 _log = logging.getLogger("limap_b200")
@@ -35,6 +37,8 @@ undistort_images = _out_of_scope("image undistortion")
 compute_sfminfos = _out_of_scope("COLMAP neighbours / ranges")
 compute_2d_bipartites_from_colmap = _out_of_scope("point-line bipartites from a COLMAP model")
 compute_exhaustive_matches = _out_of_scope("descriptor matching")
+get_hloc_keypoints = _out_of_scope("hloc keypoint correspondences")
+get_hloc_keypoints_from_log = _out_of_scope("hloc localization logs")
 
 
 def segments_folder(cfg, root):
@@ -125,3 +129,110 @@ def line_triangulation(cfg, imagecols, neighbors=None, ranges=None):
     limapio.save_obj(os.path.join(save, "triangulated_lines_nv{}.obj".format(cfg["n_visible_views"])),
                      vis.get_lines_np(n_visible_views=cfg["n_visible_views"]))
     return linetracks
+
+
+_LOC_MATCHERS = ("epipolar", "sold2", "superglue_endpoints", "gluestick", "linetr", "lbd", "l2d2")
+
+
+def _pose_line(name, pose):  # the results / pose cache line of runners/hybrid_localization.py:366-395
+    return " ".join([name] + [str(x) for x in pose.qvec] + [str(x) for x in pose.tvec]) + "\n"
+
+
+def hybrid_localization(cfg, imagecols_db, imagecols_query, point_corresp, linemap_db, retrieval, results_path,
+                        img_name_dict=None, logger=None):
+    """Visual localization of the query images of imagecols_query (runners/hybrid_localization.py:94-398): 2D-2D line
+    matches to the retrieved database images (the epipolar matcher, or a learned matcher's saved matches), 2D-3D matches
+    through the line tracks, the optional reprojection filter, then pl_estimate_absolute_pose from the coarse query pose.
+    All queries are matched in one pass over the device and solved in one lm_loc_solve launch. Writes results_path in
+    the reference's text format and returns {query id: CameraPose}. Only ransac.method None is supported."""
+    lcfg = cfg["localization"]
+    if lcfg["2d_matcher"] not in _LOC_MATCHERS:
+        raise ValueError("Unknown 2d line matcher: {}".format(lcfg["2d_matcher"]))
+    if lcfg["ransac"]["method"] is not None:  # the estimator's own error, before any work
+        estimators.pl_estimate_absolute_pose(lcfg, [], [], [], [], [], None)
+    train_ids = imagecols_db.get_img_ids()
+    query_ids = imagecols_query.get_img_ids()
+    if img_name_dict is None:
+        img_name_dict = {img_id: imagecols_db.image_name(img_id) for img_id in train_ids}
+        img_name_dict.update({img_id: imagecols_query.image_name(img_id) for img_id in query_ids})
+    id_to_name = img_name_dict
+    name_to_id = {img_name_dict[img_id]: img_id for img_id in train_ids + query_ids}
+
+    all_db_segs, _ = compute_2d_segs(cfg, imagecols_db, compute_descinfo=False)
+    all_query_segs, _ = compute_2d_segs(cfg, imagecols_query, compute_descinfo=False)
+    all_db_lines = base.get_all_lines_2d(all_db_segs)
+    all_query_lines = base.get_all_lines_2d(all_query_segs)
+    line2track = base.get_invert_idmap_from_linetracks(all_db_lines, linemap_db)
+
+    pose_dir = results_path.parent / "poses_{}".format(lcfg["2d_matcher"])
+    final_poses, todo = {}, []
+    for qid in query_ids:
+        if lcfg["skip_exists"]:
+            limapio.check_makedirs(str(pose_dir))
+            fname = os.path.join(pose_dir, f"{qid}.txt")
+            if os.path.exists(fname):
+                with open(fname) as f:
+                    data = f.read().rstrip().split("\n")[0].split()
+                    q, t = np.split(np.array(data[1:], float), [4])
+                    final_poses[qid] = base.CameraPose(q, t)
+                    continue
+        todo.append(qid)
+
+    retrieved = {qid: [name_to_id[n] for n in retrieval[id_to_name[qid]]] for qid in todo}
+    pairs_2to2 = None
+    if lcfg["2d_matcher"] != "epipolar":
+        # the learned matcher's saved matches (line2d/base_matcher.py:60-72); extraction and matching are out of scope
+        m = lcfg["2d_matcher"]
+        folder = os.path.join(cfg["dir_save"], "line_matchings", cfg["line2d"]["detector"]["method"], f"feats_{m}",
+                              "{}_n{}_top0".format(m, cfg["n_neighbors_loc"]))
+        pairs_2to2 = {}
+        for qid in todo:
+            fname = os.path.join(folder, f"matches_{qid}.npy")
+            if not os.path.exists(fname):
+                return _out_of_scope(f"2D line matching ({m}; {fname} is missing)")()
+            pairs_2to2[qid] = limapio.read_npy(fname).item()
+    query_views = {qid: imagecols_query.camview(qid) for qid in todo}
+    db_views = {t: imagecols_db.camview(t) for qid in todo for t in retrieved[qid]}
+    matches = _locfn.match_queries_to_linemap(
+        query_views, {qid: all_query_lines[qid] for qid in todo}, db_views, all_db_lines, retrieved, linemap_db,
+        line2track, IoU_threshold=lcfg["IoU_threshold"], line_pairs_2to2=pairs_2to2,
+        epipolar_filter=bool(lcfg.get("epipolar_filter")), reprojection_filter=lcfg["reprojection_filter"],
+        dist_thres=2)
+
+    # pl_estimate_absolute_pose's ransac.method None path for every query in one launch
+    jointloc_cfg = {}
+    if lcfg.get("optimize"):
+        jointloc_cfg = lcfg["optimize"].copy()
+        args = jointloc_cfg.pop("loss_func_args", None) or []
+        name = jointloc_cfg.pop("loss_func")
+        if name == "TrivialLoss":
+            args = []
+        elif name == "HuberLoss":
+            assert len(args) == 1, "HuberLoss requires one argument"
+        jointloc_cfg["loss_function"] = getattr(optimize, name)(*args)
+    if "line_weight" in lcfg:
+        jointloc_cfg["weight_point"] = 1.0
+        jointloc_cfg["weight_line"] = lcfg["line_weight"]
+    l3ds = [track.line for track in linemap_db]
+    queries = []
+    for qid in todo:
+        pairs = matches[qid]
+        if logger:
+            logger.info(f"{len(pairs)} line matches found for {len(all_query_lines[qid])} 2D lines")
+        p3ds, p2ds = point_corresp[qid]["p3ds"], point_corresp[qid]["p2ds"]
+        inl = point_corresp[qid].get("inliers")
+        if inl is not None:
+            p2ds, p3ds = np.array(p2ds)[inl], np.array(p3ds)[inl]
+        pose = imagecols_query.campose(qid)
+        queries.append(dict(l3ds=l3ds, l3d_ids=[p[1] for p in pairs], l2ds=[all_query_lines[qid][p[0]] for p in pairs],
+                            p3ds=p3ds, p2ds=p2ds, K=imagecols_query.cam(imagecols_query.camimage(qid).cam_id).K(),
+                            R=pose.R(), T=pose.T()))
+    poses, _ = optimize.solve_jointloc_batch(queries, lcfg["line_cost_func"], jointloc_cfg) if queries else ([], [])
+    for qid, pose in zip(todo, poses):
+        final_poses[qid] = pose
+        if lcfg["skip_exists"]:
+            with open(os.path.join(pose_dir, f"{qid}.txt"), "w") as f:
+                f.writelines([_pose_line(id_to_name[qid], pose)])
+    with open(results_path, "w") as f:
+        f.writelines([_pose_line(id_to_name[qid], final_poses[qid]) for qid in query_ids])
+    return final_poses
