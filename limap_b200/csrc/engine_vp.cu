@@ -95,6 +95,11 @@ int64_t lm_vp_detect_indexed(lm_ctx *c, int32_t n_images, const int64_t *line_of
   const int min_lines = 2 * std::max(cfg->min_num_supports, 10);
   bool vp_kernel_ran = false;
   if (nv > 0 && max_n >= min_lines) {
+    // the launch needs its dynamic and the kernel's static shared memory within the opt-in limit of one block
+    size_t static_smem = 0;
+    CU(lm::vp_static_smem_bytes(&static_smem));
+    if (lm::vp_smem_bytes(cfg->n_models, max_n) + static_smem > (size_t)c->max_smem_optin)
+      return fail(LM_ERR_INVALID, "n_models too large for shared memory");
     const int W = (cfg->n_models + 31) / 32;
     int grid = std::min(n_images, c->sm_count * 2);
     CU(c->d_vp_pts.ensure(16 * nv));
@@ -118,12 +123,9 @@ int64_t lm_vp_detect_indexed(lm_ctx *c, int32_t n_images, const int64_t *line_of
     p.n_images = n_images; p.n_models = cfg->n_models; p.max_n = max_n; p.min_lines = min_lines;
     p.inlier_threshold = (float)cfg->inlier_threshold;
     p.seed = cfg->seed;
-    if (lm::vp_smem_bytes(p.n_models, p.max_n) > (size_t)c->max_smem_optin)
-      return fail(LM_ERR_INVALID, "n_models too large for shared memory");
     CU(cudaEventRecord(c->evk0, s));
-    lm::launch_jlinkage(p, grid, s);
+    CU(lm::launch_jlinkage(p, grid, static_smem, s));
     CU(cudaEventRecord(c->evk1, s));
-    CU(cudaGetLastError());
     vp_kernel_ran = true;
     c->stats.n_kernel_launches += 1;
     CU(cudaMemcpyAsync(raw.data(), c->d_vp_labels.p, 4 * nv, cudaMemcpyDeviceToHost, s));

@@ -194,11 +194,23 @@ __global__ void __launch_bounds__(256) jlinkage_kernel(const __grid_constant__ V
 
 size_t vp_smem_bytes(int n_models, int max_n) { return (size_t)n_models * sizeof(float3) + (size_t)max_n * 3 + 16; }
 
-void launch_jlinkage(const VPParams &p, int grid, cudaStream_t s) {
+cudaError_t vp_static_smem_bytes(size_t *out) {
+  cudaFuncAttributes fa;
+  const cudaError_t e = cudaFuncGetAttributes(&fa, jlinkage_kernel);
+  *out = e == cudaSuccess ? fa.sharedSizeBytes : 0;
+  return e;
+}
+
+cudaError_t launch_jlinkage(const VPParams &p, int grid, size_t static_smem, cudaStream_t s) {
   const size_t smem = vp_smem_bytes(p.n_models, p.max_n);
-  if (smem > 48 * 1024) // per device: set on every launch above the default limit
-    cudaFuncSetAttribute(jlinkage_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  // the default limit of 48 KB bounds static plus dynamic shared memory; the attribute is per device, so it is set on
+  // every launch above that limit
+  if (smem + static_smem > 48 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(jlinkage_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
   jlinkage_kernel<<<grid, 256, smem, s>>>(p);
+  return cudaGetLastError();
 }
 
 } // namespace lm

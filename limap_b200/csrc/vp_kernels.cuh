@@ -17,7 +17,10 @@ struct VPParams {
   uint64_t seed;
 };
 
+// Dynamic shared memory of one launch. The kernel's static shared memory (vp_static_smem_bytes) comes on top, and the
+// two together must fit the per-block opt-in limit, and above 48 KB together the launch needs the opt-in attribute.
 size_t vp_smem_bytes(int n_models, int max_n);
-void launch_jlinkage(const VPParams &p, int grid, cudaStream_t s);
+cudaError_t vp_static_smem_bytes(size_t *out);
+cudaError_t launch_jlinkage(const VPParams &p, int grid, size_t static_smem, cudaStream_t s);
 
 } // namespace lm

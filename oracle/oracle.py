@@ -273,6 +273,10 @@ def detect_vps(line_off, segs, min_length=40.0, inlier_threshold=1.0, min_num_su
     vps = np.zeros((cap, 3))
     tot = L.orc_vp_detect_indexed(n, _p(line_off), _p(segs), C.byref(cfg), None if idx is None else _p(idx), _p(labels),
                                   _p(vp_off), _p(vps), cap)
+    if tot > cap:  # more VPs than the first guess: run again with room for all of them
+        vps = np.zeros((tot, 3))
+        L.orc_vp_detect_indexed(n, _p(line_off), _p(segs), C.byref(cfg), None if idx is None else _p(idx), _p(labels),
+                                _p(vp_off), _p(vps), tot)
     return labels, vp_off, vps[:tot]
 
 
