@@ -4,6 +4,7 @@ imported by tests/ and scripts/, never by limap_b200/.
   orc_loc_solve      the fp64 restatement of the residuals, weights, losses and LM solve, oracle/orc_loc.cpp ->
                      oracle/_build/liblimap_orc_loc.so; queries run in parallel over the host's cores
   orc_loc_functor    one residual functor on 7-wide jets (values and ambient Jacobian)
+  orc_loc_loss       the loss (Trivial, Huber, SoftLOne, Cauchy) and ScaledLoss factor of many blocks
   ref_loc_functor    the reference's own ReprojectionLineFunctor / ReprojectionPointFunctor (cost_functions.h, compiled
                      unchanged by oracle/ref_loc.cpp) on 7-wide jets -> oracle/_ref/liblimap_ref_loc.so; built only where
                      the reference source tree exists, used to write tests/golden/ref/localization.npz"""
@@ -59,6 +60,8 @@ def lib():
         L.orc_loc_solve.argtypes = [C.c_int64] + [_P] * 10 + [_P, C.c_int32] + [_P] * 6
         L.orc_loc_functor.restype = None
         L.orc_loc_functor.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int] + [_P] * 6
+        L.orc_loc_loss.restype = None
+        L.orc_loc_loss.argtypes = [C.c_int, C.c_double, C.c_int64, _P, _P, _P]
         _lib = L
     return _lib
 
@@ -112,3 +115,12 @@ def functor(kind, data, kvec, qvec, tvec, cost_function=2, weight_function=0, us
     fn(kind, cost_function, weight_function, int(use3d), _ptr(f64(data)), _ptr(f64(kvec)), _ptr(f64(qvec)),
        _ptr(f64(tvec)), _ptr(res), _ptr(jac))
     return res, jac
+
+
+def loss(kind, scale, a, s):
+    """rho[n][3] of the loss (kind 0..3, scale) with ScaledLoss factors a[n] at squared residual norms s[n]."""
+    s = np.ascontiguousarray(s, np.float64).ravel()
+    a = np.ascontiguousarray(np.broadcast_to(a, s.shape), np.float64)
+    rho = np.zeros((len(s), 3))
+    lib().orc_loc_loss(kind, scale, len(s), _ptr(a), _ptr(s), _ptr(rho))
+    return rho

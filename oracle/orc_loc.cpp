@@ -245,6 +245,11 @@ void orc_loc_functor(int kind, int cf, int wf, int use3d, const double *data, co
   }
 }
 
+// The loss of n blocks with squared residual norms s[n] and ScaledLoss factors a[n]: rho[n][3].
+void orc_loc_loss(int kind, double scale, int64_t n, const double *a, const double *s, double *rho) {
+  for (int64_t i = 0; i < n; ++i) orc::loss_eval(kind, scale, a[i], s[i], rho + 3 * i);
+}
+
 // The same functor in plain doubles (the path Ceres takes when it evaluates a cost without Jacobians).
 void orc_loc_functor_value(int kind, int cf, int wf, int use3d, const double *data, const double *kvec,
                            const double *qvec, const double *tvec, double *res) {
